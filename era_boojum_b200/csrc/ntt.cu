@@ -342,20 +342,26 @@ static int32_t get_pow_tables(bj_ctx* ctx, u64 c, int log_n, u64 scale, PowTab* 
 
 int32_t get_pow_tables_public(bj_ctx* ctx, u64 c, int log_n, u64 scale, PowTab* out) { return get_pow_tables(ctx, c, log_n, scale, out); }
 
+// The largest plan of any allowed tile setting (BJ_NTT_MAX_TILE_LOG 8..14) up to log_n = 32: an inverse of 2^31 or 2^32
+// with 2^8-value tiles takes 6 passes (tools/ntt_model.py enumerates them).
+static constexpr int NTT_MAX_PASSES = 6;
+
 struct Plan {
   int n_pass;
-  int t[4];
-  int w[4];
+  int t[NTT_MAX_PASSES];
+  int w[NTT_MAX_PASSES];
 };
 
-static Plan make_plan(const bj_ctx* ctx, int m, bool transpose_last) {
-  Plan pl{};
+// false when the plan would need more than NTT_MAX_PASSES passes (pl->n_pass is set, the arrays are not)
+static bool make_plan(const bj_ctx* ctx, int m, bool transpose_last, Plan* out) {
+  Plan& pl = *out;
+  pl = Plan{};
   const int MAXE = ctx->ntt_max_tile_log;
   if (m <= 12) {
     pl.n_pass = 1;
     pl.t[0] = m;
     pl.w[0] = 0;
-    return pl;
+    return true;
   }
   // tiles of at most 2^MAXE values (default 2^13 = 68 KB of shared memory -> 3 CTAs per SM); the transposing last pass
   // keeps at least 4 columns so that its stores are 32-byte segments
@@ -365,6 +371,7 @@ static Plan make_plan(const bj_ctx* ctx, int m, bool transpose_last) {
   int rest = m - t_last;
   int n_front = (rest + TM - 1) / TM;
   pl.n_pass = n_front + 1;
+  if (pl.n_pass > NTT_MAX_PASSES) return false;
   int r0 = 0;
   for (int i = 0; i < n_front; i++) {
     int ti = rest / (n_front - i);
@@ -379,21 +386,40 @@ static Plan make_plan(const bj_ctx* ctx, int m, bool transpose_last) {
   }
   pl.t[n_front] = t_last;
   pl.w[n_front] = transpose_last ? std::min(std::min(MAXE - t_last, 5), r0) : 0;
-  return pl;
+  return true;
+}
+
+// grid.y limit: a batch of more columns is launched in slices of at most this many columns
+static constexpr u32 MAX_GRID_Y = 65535;
+
+// Launches `fn` over the batch in column slices of at most MAX_GRID_Y columns, each slice with src / dst moved to its
+// first column.  Even strides keep the 16-byte alignment the specialised kernels need.
+template <typename F>
+static int32_t launch_column_slices(bj_ctx* ctx, const NttPass& p, u32 n_cols, F&& fn) {
+  for (u32 c0 = 0; c0 < n_cols; c0 += std::min(MAX_GRID_Y, n_cols - c0)) {
+    NttPass ps = p;
+    ps.src = p.src + (u64)c0 * p.src_col_stride;
+    ps.dst = p.dst + (u64)c0 * p.dst_col_stride;
+    fn(ps, std::min(MAX_GRID_Y, n_cols - c0));
+    BJ_LAUNCH_CHECK(ctx);
+  }
+  return BJ_OK;
 }
 
 static int32_t launch_pass(bj_ctx* ctx, const NttPass& p, u32 n_cols) {
   const int LOG_E = p.t + p.w;
   const u64 tiles = p.kind == PASS_TILE ? (1ull << (p.log_n - p.t - p.w)) : (1ull << (p.r0 - p.w));
-  if (tiles > 0x7fffffffull || n_cols > 65535) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "grid too large");
-  dim3 grid((unsigned)tiles, n_cols, 1);
+  if (tiles > 0x7fffffffull) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "grid too large");
   // specialised kernel when one is instantiated for this tile shape and the buffers allow 128-bit accesses
   V2Launch v2;
   const bool aligned = ((((uintptr_t)p.src | (uintptr_t)p.dst) & 15) == 0) && ((p.src_col_stride | p.dst_col_stride) & 1) == 0;
+  // the specialised one-column tiles (w = 0) move pairs of adjacent rows, so they serve contiguous (last) passes only; a
+  // front pass with w = 0 (BJ_NTT_PASS1_W=0) has strided rows and takes the generic kernel
+  const bool v2_shape_ok = !(p.kind == PASS_TILE && p.w == 0 && p.log_n - p.r0 - p.t != 0);
   // experiment: bulk-copy (TMA) staged contiguous pass, BJ_NTT_BULK=1 (ntt_v2.cuh)
   const bool bulk_ok = ctx->ntt_bulk && aligned && p.kind == PASS_TILE && p.w == 0 && p.scale_mode == SCALE_NONE &&
                        p.log_n - p.r0 - p.t == 0 && ((p.src_col_stride | p.dst_col_stride) & 15) == 0;
-  if (ctx->ntt_use_v2 && aligned && ((bulk_ok && v2_bulk_lookup(p.t, &v2)) || v2_lookup(p.t, p.w, p.kind, &v2))) {
+  if (ctx->ntt_use_v2 && aligned && v2_shape_ok && ((bulk_ok && v2_bulk_lookup(p.t, &v2)) || v2_lookup(p.t, p.w, p.kind, &v2))) {
     bool known = false;
     for (void* f : ctx->attr_done) known |= (f == (void*)v2.fn);
     if (!known) {
@@ -402,9 +428,9 @@ static int32_t launch_pass(bj_ctx* ctx, const NttPass& p, u32 n_cols) {
                                         cudaSharedmemCarveoutMaxShared));
       ctx->attr_done.push_back((void*)v2.fn);
     }
-    v2.fn<<<grid, v2.threads, v2.smem, ctx->stream>>>(p);
-    BJ_LAUNCH_CHECK(ctx);
-    return BJ_OK;
+    return launch_column_slices(ctx, p, n_cols, [&](const NttPass& ps, u32 cols) {
+      v2.fn<<<dim3((unsigned)tiles, cols, 1), v2.threads, v2.smem, ctx->stream>>>(ps);
+    });
   }
   const int threads = std::max(32, std::min(512, (1 << LOG_E) >> 4));
   const size_t smem = sizeof(u64) * ((size_t)(1 << LOG_E) + ((size_t)(1 << LOG_E) >> 4) + 1);
@@ -414,9 +440,9 @@ static int32_t launch_pass(bj_ctx* ctx, const NttPass& p, u32 n_cols) {
                                       cudaSharedmemCarveoutMaxShared));
     ctx->ntt_attr_set = true;
   }
-  ntt_pass_kernel<<<grid, threads, smem, ctx->stream>>>(p);
-  BJ_LAUNCH_CHECK(ctx);
-  return BJ_OK;
+  return launch_column_slices(ctx, p, n_cols, [&](const NttPass& ps, u32 cols) {
+    ntt_pass_kernel<<<dim3((unsigned)tiles, cols, 1), threads, smem, ctx->stream>>>(ps);
+  });
 }
 
 // One batched transform.  src may equal dst for forward; the natural->natural inverse with more than one
@@ -439,7 +465,8 @@ static int32_t run_transform(bj_ctx* ctx, const u64* src, u64 src_stride, u64* d
     BJ_LAUNCH_CHECK(ctx);
     return BJ_OK;
   }
-  const Plan pl = make_plan(ctx, m, inverse);
+  Plan pl;
+  if (!make_plan(ctx, m, inverse, &pl)) BJ_FAIL(ctx, BJ_ERR_UNSUPPORTED, "NTT plan needs more passes than NTT_MAX_PASSES");
   PowTab pt{};
   int scale_mode = SCALE_NONE;
   u64 scale_const = 1;
@@ -532,7 +559,11 @@ static int32_t run_transform(bj_ctx* ctx, const u64* src, u64 src_stride, u64* d
   return BJ_OK;
 }
 
-static bool inverse_needs_scratch(const bj_ctx* ctx, int m) { return m >= 4 && make_plan(ctx, m, true).n_pass > 1; }
+static bool inverse_needs_scratch(const bj_ctx* ctx, int m) {
+  Plan pl;
+  make_plan(ctx, m, true, &pl);  // n_pass is set even when the plan is refused; run_transform reports that
+  return m >= 4 && pl.n_pass > 1;
+}
 
 }  // namespace bj
 
@@ -586,9 +617,12 @@ int32_t bj_bitreverse(bj_ctx* ctx, uint64_t* d_data, uint32_t log_n, uint32_t n_
   if (!ctx || !d_data || log_n > 40) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_bitreverse: bad argument");
   if (n_cols == 0 || log_n == 0) return BJ_OK;
   const u64 n = 1ull << log_n;
-  dim3 grid((unsigned)((n + 255) / 256), n_cols);
-  bitreverse_kernel<<<grid, 256, 0, ctx->stream>>>((u64*)d_data, col_stride, (int)log_n);
-  BJ_LAUNCH_CHECK(ctx);
+  if ((n + 255) / 256 > 0x7fffffffull) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_bitreverse: grid too large");
+  for (u32 c0 = 0; c0 < n_cols; c0 += std::min(MAX_GRID_Y, n_cols - c0)) {  // grid.y slices, as in launch_pass
+    dim3 grid((unsigned)((n + 255) / 256), std::min(MAX_GRID_Y, n_cols - c0));
+    bitreverse_kernel<<<grid, 256, 0, ctx->stream>>>((u64*)d_data + (u64)c0 * col_stride, col_stride, (int)log_n);
+    BJ_LAUNCH_CHECK(ctx);
+  }
   return BJ_OK;
 }
 

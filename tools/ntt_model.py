@@ -30,6 +30,9 @@ def twiddle_table(log_n, inverse):
     return [pow(w, brev(k, bits), P) for k in range(1 << bits)] if log_n >= 1 else [1]
 
 
+NTT_MAX_PASSES = 6  # capacity of ntt.cu's Plan
+
+
 def make_plan(m, transpose_last, MAXE=13, pass1_w=-1):
     if m <= 12:
         return [(m, 0)]
@@ -38,6 +41,8 @@ def make_plan(m, transpose_last, MAXE=13, pass1_w=-1):
     t_last = min(TL, max((m + 1) // 2, m - 10))
     rest = m - t_last
     n_front = (rest + TM - 1) // TM
+    if n_front + 1 > NTT_MAX_PASSES:
+        raise ValueError("plan of 2^%d (MAXE %d) needs %d passes" % (m, MAXE, n_front + 1))
     plan, r0 = [], 0
     for i in range(n_front):
         ti = rest // (n_front - i)
