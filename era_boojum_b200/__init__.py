@@ -68,6 +68,11 @@ def _ok(status, what="libboojum_b200 call"):
         raise BoojumError(status, "%s: %s" % (what, lib.bj_status_string(status).decode()))
 
 
+def _shard_split(world, lde_degree):
+    """log2 of the row blocks per coset of a domain shard of `world` ranks (0: every rank holds whole cosets)"""
+    return max(0, world.bit_length() - lde_degree.bit_length())
+
+
 class FriOracles:
     """FriOracles (cs/implementations/fri/mod.rs:36-47): base + intermediate oracle caps, monomial forms, queries."""
 
@@ -217,13 +222,20 @@ class Context:
     def synchronize(self):
         self._check(lib.bj_ctx_synchronize(self._h))
 
-    shard_rank, shard_world = 0, 1
+    shard_rank, shard_world, shard_split = 0, 1, 0
 
     def set_coset_shard(self, rank, world, lde_degree):
         """bj_ctx_set_coset_shard: this context holds the LDE cosets j = rank (mod world) of every committed polynomial
         (multi-GPU proving, one process per GPU).  Sizes passed to the C-ABI stay global; tensors are local."""
         self._check(lib.bj_ctx_set_coset_shard(self._h, rank, world, lde_degree.bit_length() - 1))
+        self.shard_rank, self.shard_world, self.shard_split = rank, world, 0
+
+    def set_domain_shard(self, rank, world, lde_degree):
+        """bj_ctx_set_domain_shard: set_coset_shard for world <= lde_degree; above it every coset is cut into
+        B = world / lde_degree row blocks (units) and this context holds the units u = rank (mod world), [local unit][n / B]."""
+        self._check(lib.bj_ctx_set_domain_shard(self._h, rank, world, lde_degree.bit_length() - 1))
         self.shard_rank, self.shard_world = rank, world
+        self.shard_split = _shard_split(world, lde_degree)
 
     def launch_count(self):
         return int(lib.bj_launch_count(self._h))
@@ -261,13 +273,18 @@ class Context:
         self._check(lib.bj_bitreverse(self._h, self._ptr(cols), log_n, n_cols, n))
         return cols
 
-    def transform_raw_storages_to_lde(self, cols, lde_degree, from_monomials=False, out=None):
-        """[n_cols, n] Lagrange values -> [n_cols, lde_degree, n] (coset-major, bit-reversed in coset)."""
+    def transform_raw_storages_to_lde(self, cols, lde_degree, from_monomials=False, out=None, next_row=False):
+        """[n_cols, n] Lagrange values -> [n_cols, lde_degree, n] (coset-major, bit-reversed in coset).  A shard produces
+        only its own units: [n_cols, (lde_degree * B) // world, n // B] with B row blocks per coset (B = 1: whole cosets).
+        next_row: the LDE of f(w_n x) instead (bj_lde_next_row)."""
         log_n, n_cols, n = self._cols(cols)
         log_l = lde_degree.bit_length() - 1
-        if out is None:   # a coset shard produces only its own lde_degree / world cosets
-            out = self._torch.empty((n_cols, lde_degree // self.shard_world, n), dtype=self._torch.int64, device=cols.device)
-        self._check(lib.bj_lde(self._h, self._ptr(cols), n, self._ptr(out), log_n, log_l, n_cols, int(from_monomials)))
+        if out is None:
+            b = 1 << self.shard_split
+            out = self._torch.empty((n_cols, max(1, lde_degree * b // self.shard_world), n // b), dtype=self._torch.int64,
+                                    device=cols.device)
+        fn = lib.bj_lde_next_row if next_row else lib.bj_lde
+        self._check(fn(self._h, self._ptr(cols), n, self._ptr(out), log_n, log_l, n_cols, int(from_monomials)))
         return out
 
     # ---- Merkle ----
@@ -548,7 +565,7 @@ class Comm:
 
     def __init__(self, ctx, handle, rank, world, lde_degree):
         self.ctx, self._h, self.rank, self.world = ctx, handle, rank, world
-        ctx.shard_rank, ctx.shard_world = rank, world
+        ctx.shard_rank, ctx.shard_world, ctx.shard_split = rank, world, _shard_split(world, lde_degree)
         ctx._children.add(self)
 
     @staticmethod
@@ -609,7 +626,7 @@ class Comm:
         if getattr(self, "_h", None):
             lib.bj_comm_destroy(self._h)
             self._h = None
-            self.ctx.shard_rank, self.ctx.shard_world = 0, 1
+            self.ctx.shard_rank, self.ctx.shard_world, self.ctx.shard_split = 0, 1, 0
 
     def __del__(self):
         try:

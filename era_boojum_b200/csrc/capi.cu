@@ -210,6 +210,21 @@ int32_t bj_ctx_set_coset_shard(bj_ctx* ctx, uint32_t rank, uint32_t world, uint3
   ctx->shard_log_lde = log_lde;
   ctx->shard.first = rank;
   ctx->shard.log_stride = ls;
+  ctx->shard.log_split = 0;
+  return BJ_OK;
+}
+
+int32_t bj_ctx_set_domain_shard(bj_ctx* ctx, uint32_t rank, uint32_t world, uint32_t log_lde) {
+  bj::DeviceGuard device_guard(ctx);
+  if (!ctx) return BJ_ERR_INVALID_ARG;
+  if (world == 0 || (world & (world - 1)) || rank >= world || log_lde > 16 || world > (8u << log_lde))
+    BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_ctx_set_domain_shard: world must be a power of two <= 8 * the LDE factor and rank < world");
+  uint32_t ls = 0;
+  while ((1u << ls) < world) ls++;
+  ctx->shard_log_lde = log_lde;
+  ctx->shard.first = rank;
+  ctx->shard.log_stride = ls;
+  ctx->shard.log_split = ls > log_lde ? ls - log_lde : 0;  // row blocks per coset when there are more ranks than cosets
   return BJ_OK;
 }
 

@@ -232,13 +232,15 @@ int32_t comm_assemble_cap(bj_ctx* ctx, const u64* h_local_cap, uint32_t cap_size
     if (h_local_cap != h_global_cap) memcpy(h_global_cap, h_local_cap, sizeof(u64) * 4 * cap_size);
     return BJ_OK;
   }
-  if (cap_size < lde_factor || lde_factor % world) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "sharded proving needs cap_size >= LDE factor and world | LDE factor");
-  const uint32_t per = cap_size / lde_factor, local = cap_size / world;
+  // every unit (a coset, or a row block of one) is a whole subtree: `per` cap nodes
+  const uint32_t units = lde_factor << ctx->shard.log_split;
+  if (cap_size < units || units % world) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "sharded proving needs cap_size >= LDE factor * row blocks and world | units");
+  const uint32_t per = cap_size / units, local = cap_size / world;
   std::vector<u64> all((size_t)4 * cap_size);
   BJ_TRY(comm_all_gather_host(ctx->comm, h_local_cap, all.data(), (u64)4 * local));
   for (uint32_t r = 0; r < world; r++)
-    for (uint32_t k = 0; k < lde_factor / world; k++) {
-      const uint32_t j = k * world + r;
+    for (uint32_t k = 0; k < units / world; k++) {
+      const u64 j = ctx->shard.unit_of(r, k);
       memcpy(h_global_cap + (size_t)4 * j * per, all.data() + (size_t)4 * (r * local + k * per), sizeof(u64) * 4 * per);
     }
   return BJ_OK;
@@ -262,8 +264,9 @@ int32_t bj_comm_unique_id(uint8_t out[BJ_COMM_UNIQUE_ID_BYTES]) {
 }
 
 static int32_t comm_attach(bj_ctx* ctx, bj_comm* c, uint32_t log_lde) {
-  // the communicator defines the coset shard of its context: rank r keeps the cosets j = r (mod world)
-  BJ_TRY(bj_ctx_set_coset_shard(ctx, c->rank, c->world, log_lde));
+  // the communicator defines the domain shard of its context: rank r keeps the units u = r (mod world) - the cosets
+  // j = r (mod world) for world <= the LDE factor, row blocks of cosets above it
+  BJ_TRY(bj_ctx_set_domain_shard(ctx, c->rank, c->world, log_lde));
   ctx->comm = c;
   return BJ_OK;
 }

@@ -12,6 +12,7 @@
 
 namespace bj {
 using gl::u64;
+using gl::u32;
 
 struct PowTab {
   u64 coset;
@@ -23,22 +24,54 @@ struct PowTab {
   u64* full;  // s * c^i for all i < 2^log_n, or nullptr (built while the per-context budget lasts)
 };
 
-// Coset shard of a multi-GPU prover: LDE-domain buffers of this context hold only the cosets j = first + k * 2^log_stride
-// (k = 0, 1, ...), stored [local coset k][row].  A local flat index [k | i] maps to the global index [k | first | i].
+// Domain shard of a multi-GPU prover, the one owner of the layout rule.  The LDE domain is cut into UNITS u = j * B + p,
+// B = 2^log_split: row block p (rows [p n / B, (p + 1) n / B) of the coset's bit-reversed row order) of coset j, so the flat
+// index of a domain point is t = u * (n / B) + i'.  LDE-domain buffers of this context hold only the units
+// u = first + k * 2^log_stride (k = 0, 1, ...), stored [local unit k][n / B rows]: a local flat index [k | i'] maps to the
+// global index [k | first | i'].  log_split = 0 is the coset shard (a unit is a whole coset).  The first L * B units of any
+// factor D >= L are the factor-L domain, so the quotient's wider domain shards the same way as the committed one.
 struct CosetShard {
   uint32_t first = 0;
-  uint32_t log_stride = 0;
+  uint32_t log_stride = 0;  // log2(world)
+  uint32_t log_split = 0;   // log2(B), row blocks per coset
   __host__ __device__ __forceinline__ u64 global_index(u64 t_loc, int log_coset_len) const {
     if (log_stride == 0) return t_loc;
-    const u64 i = t_loc & ((1ull << log_coset_len) - 1);
-    const u64 k = t_loc >> log_coset_len;
-    return ((((k << log_stride) | first)) << log_coset_len) | i;
+    const int lu = log_coset_len - (int)log_split;
+    const u64 i = t_loc & ((1ull << lu) - 1);
+    const u64 k = t_loc >> lu;
+    return ((((k << log_stride) | first)) << lu) | i;
   }
-  // how many of the first `group` (power of two) global cosets are local
-  __host__ __device__ __forceinline__ u64 local_cosets(u64 group) const {
-    const u64 stride = 1ull << log_stride;
+  // global unit held by `rank` in its local slot k
+  __host__ __device__ __forceinline__ u64 unit_of(u64 rank, u64 k) const { return (k << log_stride) | rank; }
+  __host__ __device__ __forceinline__ u64 global_unit(u64 k) const { return unit_of(first, k); }
+  // how many units of the first `cosets` (power of two) global cosets are local
+  __host__ __device__ __forceinline__ u64 local_units(u64 cosets) const {
+    const u64 stride = 1ull << log_stride, group = cosets << log_split;
     if (group >= stride) return group >> log_stride;
     return first < group ? 1 : 0;
+  }
+  // local points of the first `cosets` cosets of 2^log_coset_len rows
+  __host__ __device__ __forceinline__ u64 local_points(u64 cosets, int log_coset_len) const {
+    return local_units(cosets) << (log_coset_len - (int)log_split);
+  }
+  // rank that holds the global flat index t, and t's index in that rank's local layout
+  __host__ __device__ __forceinline__ u32 owner(u64 t, int log_coset_len) const {
+    return (u32)((t >> (log_coset_len - (int)log_split)) & ((1ull << log_stride) - 1));
+  }
+  __host__ __device__ __forceinline__ u64 owner_index(u64 t, int log_coset_len) const {
+    const int lu = log_coset_len - (int)log_split;
+    return (((t >> lu) >> log_stride) << lu) | (t & ((1ull << lu) - 1));
+  }
+  // shift sigma of global unit u on the factor-2^log_lde LDE of 2^log_n rows: its points are sigma * w_{n/B}^{bitrev(i')},
+  // sigma = c_j * w_n^{bitrev_s(p)} with c_j = 7 * w_{nL}^{bitrev_L(j)} the shift of coset j
+  __host__ u64 unit_shift(u64 u, u32 log_n, u32 log_lde) const {
+    const u64 j = u >> log_split, p = u & ((1ull << log_split) - 1);
+    u64 jr = 0, pr = 0;
+    for (u32 b = 0; b < log_lde; b++) jr |= ((j >> b) & 1) << (log_lde - 1 - b);
+    for (u32 b = 0; b < log_split; b++) pr |= ((p >> b) & 1) << (log_split - 1 - b);
+    u64 s = gl::mul(gl::MULT_GEN, gl::pow(gl::omega(log_n + log_lde), jr));
+    if (log_split) s = gl::mul(s, gl::pow(gl::omega(log_n), pr));
+    return s;
   }
 };
 
@@ -88,7 +121,7 @@ struct bj_ctx {
   size_t l2_window_max = 0;      // largest access-policy window the device accepts
   int ntt_bulk = 0;              // BJ_NTT_BULK=1: experiment, bulk-copy (TMA) staged contiguous pass (ntt_v2.cuh)
   cudaMemPool_t pool = nullptr;  // private stream-ordered pool of the prover driver (keeps freed blocks: no OS round trips per proof)
-  bj::CosetShard shard;  // bj_ctx_set_coset_shard; default = the whole domain
+  bj::CosetShard shard;  // bj_ctx_set_coset_shard / bj_ctx_set_domain_shard; default = the whole domain
   uint32_t shard_log_lde = 0;  // LDE factor the shard was declared for (locates the coset bits of flat indices)
 };
 
@@ -152,8 +185,8 @@ int32_t comm_wait(bj_comm* c, cudaEvent_t done);
 int32_t comm_broadcast_host(bj_comm* c, u64* h_buf, u64 n, uint32_t root);
 uint32_t comm_world(const bj_ctx* ctx);
 uint32_t comm_rank(const bj_ctx* ctx);
-// global cap (cap_size digests) of an oracle whose local tree (this rank's cosets [k][row]) ends in cap_size / world digests:
-// cap node c of the global tree belongs to coset c / (cap_size / L) (leaf index = coset * n + row, proof.rs:89-91)
+// global cap (cap_size digests) of an oracle whose local tree (this rank's units [k][row]) ends in cap_size / world digests:
+// cap node c of the global tree belongs to unit c / (cap_size / (L * B)) (leaf index = coset * n + row, proof.rs:89-91)
 int32_t comm_assemble_cap(bj_ctx* ctx, const u64* h_local_cap, uint32_t cap_size, uint32_t lde_factor, u64* h_global_cap);
 int32_t ensure_twiddles(bj_ctx* ctx, int log_n);
 int32_t param_upload(bj_ctx* ctx, const void* host, size_t bytes, void** d_out);

@@ -113,7 +113,7 @@ struct DeepColumn {
 struct DeepParams {
   const DeepColumn* cols;
   u32 n_cols;
-  u64 n_rows;                // n * (local cosets)
+  u64 n_rows;                // local points: (local units) * (rows per unit)
   int log_n;                 // coset length (locates the coset bits when the context holds a coset shard)
   CosetShard shard;
   const u64* tab;            // forward twiddles of the whole LDE domain
@@ -296,9 +296,10 @@ int32_t bj_deep_quotient_group(bj_ctx* ctx, const uint64_t* const* h_src_c0, con
   p.log_n = (int)log_rows;
   p.shard = ctx->shard;
   if (ctx->shard.log_stride) {
-    if (log_rows < ctx->shard_log_lde + 1) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_deep_quotient_group: domain smaller than the sharded LDE factor");
+    if (log_rows < ctx->shard_log_lde + ctx->shard.log_split + 1)
+      BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_deep_quotient_group: domain smaller than the units of the shard");
     p.log_n = (int)(log_rows - ctx->shard_log_lde);
-    p.n_rows = ctx->shard.local_cosets(1ull << ctx->shard_log_lde) << p.log_n;
+    p.n_rows = ctx->shard.local_points(1ull << ctx->shard_log_lde, p.log_n);
   }
   p.tab = ctx->tw_fwd;
   p.at = {gl::canon(h_at[0]), gl::canon(h_at[1])};

@@ -66,7 +66,6 @@ extern "C" int32_t bj_fri_fold(bj_ctx* ctx, const uint64_t* d_c0, const uint64_t
   if (log_fold < 1 || log_fold > 3 || log_fold > log_m || log_m > 32)
     BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_fri_fold: log_fold must be 1..3 and <= log_m");
   if (((uintptr_t)d_c0 | (uintptr_t)d_c1) & 15) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_fri_fold: inputs must be 16-byte aligned");
-  BJ_TRY(ensure_twiddles(ctx, (int)log_m));
   FoldParams fp;
   gl::e2 a = {gl::canon(h_alpha[0]), gl::canon(h_alpha[1])};
   u64 kappa = gl::canon(*h_coset_inv_io);
@@ -82,11 +81,13 @@ extern "C" int32_t bj_fri_fold(bj_ctx* ctx, const uint64_t* d_c0, const uint64_t
   fp.shard = ctx->shard;
   fp.log_coset_out = 0;
   if (ctx->shard.log_stride) {
-    // local vectors hold the owned cosets only; a fold never crosses a coset while the folded coset is >= 1 element
-    if (log_m < ctx->shard_log_lde + log_fold) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_fri_fold: fold would cross cosets of the shard");
+    // local vectors hold the owned units only; a fold never crosses a unit while the folded unit is >= 1 element
+    if (log_m < ctx->shard_log_lde + ctx->shard.log_split + log_fold)
+      BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_fri_fold: fold would cross units of the shard");
     fp.log_coset_out = (int)(log_m - log_fold - ctx->shard_log_lde);
-    n_out = ctx->shard.local_cosets(1ull << ctx->shard_log_lde) << fp.log_coset_out;
+    n_out = ctx->shard.local_points(1ull << ctx->shard_log_lde, fp.log_coset_out);
   }
+  BJ_TRY(ensure_twiddles(ctx, (int)log_m));
   const unsigned blocks = (unsigned)((n_out + 255) / 256);
   const u64* roots = ctx->tw_inv;
   switch (log_fold) {

@@ -171,14 +171,14 @@ int32_t bj_do_fri_with_hasher(bj_ctx* ctx, bj_transcript* transcript, const uint
   const u64* cur0 = (const u64*)d_c0;
   const u64* cur1 = (const u64*)d_c1;
   u32 log_m = log_full_size;
-  // coset-sharded context: the codewords hold this rank's cosets only ([local coset][row], 1 / world of every vector); folds and
-  // oracle subtrees are local (a fold of 2^k neighbours never leaves a coset), caps are assembled across the ranks so that all
+  // sharded context: the codewords hold this rank's units only ([local unit][row], 1 / world of every vector); folds and
+  // oracle subtrees are local (a fold of 2^k neighbours never leaves a unit), caps are assembled across the ranks so that all
   // of them draw the same challenges, and the last codeword (a few hundred elements) is gathered and interpolated everywhere
   const u32 world = comm_world(ctx);
   u32 log_world = 0;
   while ((1u << log_world) < world) log_world++;
-  if (world > 1 && (log_lde != ctx->shard_log_lde || cap_size < (1u << log_lde)))
-    BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_do_fri: sharded FRI needs cap_size >= LDE factor and the LDE factor of the shard");
+  if (world > 1 && (log_lde != ctx->shard_log_lde || cap_size < std::max(1u << log_lde, world)))
+    BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_do_fri: sharded FRI needs cap_size >= max(LDE factor, world) and the LDE factor of the shard");
   const u32 cap_local = cap_size / world;
   for (u32 i = 0; i < n_schedule; i++) {
     const u32 k = schedule[i];
@@ -238,8 +238,10 @@ int32_t bj_do_fri_with_hasher(bj_ctx* ctx, bj_transcript* transcript, const uint
     BJ_CUDA(ctx, cudaMemcpyAsync(f0.p, cur0, sizeof(u64) * fft_size, cudaMemcpyDeviceToDevice, ctx->stream));
     BJ_CUDA(ctx, cudaMemcpyAsync(f1.p, cur1, sizeof(u64) * fft_size, cudaMemcpyDeviceToDevice, ctx->stream));
   } else {
-    // local [L / world][mc] (c0 | c1) from every rank -> global [L][mc]: coset slot k of rank r is coset k * world + r
-    const u64 loc = fft_size / world, mc = fft_size >> log_lde, l_loc = (1ull << log_lde) / world;
+    // local [units / world][mc] (c0 | c1) from every rank -> global [units][mc]: unit slot kk of rank r is unit j below
+    const u64 units = (1ull << log_lde) << ctx->shard.log_split;
+    const u64 loc = fft_size / world, mc = fft_size / units, u_loc = units / world;
+    if (mc == 0) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_do_fri: the last codeword is shorter than the units of the shard");
     DevBuf snd, rcv;
     BJ_TRY(snd.alloc(ctx, sizeof(u64) * 2 * loc));
     BJ_TRY(rcv.alloc(ctx, sizeof(u64) * 2 * fft_size));
@@ -247,8 +249,8 @@ int32_t bj_do_fri_with_hasher(bj_ctx* ctx, bj_transcript* transcript, const uint
     BJ_CUDA(ctx, cudaMemcpyAsync(snd.u() + loc, cur1, sizeof(u64) * loc, cudaMemcpyDeviceToDevice, ctx->stream));
     BJ_TRY(comm_all_gather(ctx->comm, snd.u(), rcv.u(), 2 * loc));
     for (u32 r = 0; r < world; r++)
-      for (u64 kk = 0; kk < l_loc; kk++) {
-        const u64 j = kk * world + r;
+      for (u64 kk = 0; kk < u_loc; kk++) {
+        const u64 j = ctx->shard.unit_of(r, kk);
         BJ_CUDA(ctx, cudaMemcpyAsync((u64*)f0.p + j * mc, rcv.u() + (u64)r * 2 * loc + kk * mc, sizeof(u64) * mc, cudaMemcpyDeviceToDevice, ctx->stream));
         BJ_CUDA(ctx, cudaMemcpyAsync((u64*)f1.p + j * mc, rcv.u() + (u64)r * 2 * loc + loc + kk * mc, sizeof(u64) * mc, cudaMemcpyDeviceToDevice, ctx->stream));
       }

@@ -626,24 +626,81 @@ int32_t bj_bitreverse(bj_ctx* ctx, uint64_t* d_data, uint32_t log_n, uint32_t n_
   return BJ_OK;
 }
 
-int32_t bj_lde(bj_ctx* ctx, const uint64_t* d_in, uint64_t in_col_stride, uint64_t* d_out, uint32_t log_n,
-               uint32_t log_lde, uint32_t n_cols, int32_t from_monomials) {
-  bj::DeviceGuard device_guard(ctx);
+}  // extern "C"
+
+namespace bj {
+
+struct UnitPowers {
+  u64 v[8];  // sigma^(m * n / B), m < B
+};
+
+// Fold of a coefficient vector onto a row block: on the points of a unit with shift sigma, x^(n/B) = sigma^(n/B), so
+// f(x) = sum_{k < n/B} b_k x^k with b_k = sum_{m < B} sigma^(m n / B) a_{k + m n / B}.
+// b[c][k] for c < cnt columns (a: column stride a_stride, b: column stride b_stride).
+__global__ void __launch_bounds__(256) lde_unit_fold_kernel(const u64* __restrict__ a, u64 a_stride, u64* __restrict__ b, u64 b_stride,
+                                                             int log_nb, u32 n_blocks, u64 total, UnitPowers pw) {
+  const u64 idx = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const u64 c = idx >> log_nb, k = idx & ((1ull << log_nb) - 1);
+  const u64* src = a + c * a_stride + k;
+  u64 acc = gl::canon(src[0]);
+  for (u32 m = 1; m < n_blocks; m++) acc = gl::add(acc, gl::canon(gl::mul(src[(u64)m << log_nb], pw.v[m])));  // any u64 input
+  b[c * b_stride + k] = gl::canon(acc);
+}
+
+// bj_lde, and with next_row the LDE of f(w_n x) (every unit shift times w_n, same row order)
+static int32_t lde_impl(bj_ctx* ctx, const uint64_t* d_in, uint64_t in_col_stride, uint64_t* d_out, uint32_t log_n, uint32_t log_lde,
+                        uint32_t n_cols, int32_t from_monomials, bool next_row) {
   if (!ctx || !d_in || !d_out || log_n + log_lde > 32 || in_col_stride < (1ull << log_n))
     BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_lde: bad argument");
   if (n_cols == 0) return BJ_OK;
   const u64 n = 1ull << log_n, L = 1ull << log_lde;
-  // a coset shard owns the cosets j = first (mod world) of ANY factor >= world (the first L cosets of a larger domain are the
-  // factor-L domain), so the quotient's wider evaluation domain shards the same way as the committed one
-  if (ctx->shard.log_stride > log_lde)
+  // a shard owns the units u = first (mod world) of ANY factor with at least `world` units (the first L cosets of a larger
+  // domain are the factor-L domain), so the quotient's wider evaluation domain shards the same way as the committed one
+  const u32 s = ctx->shard.log_split;
+  if (ctx->shard.log_stride > log_lde + s)
     BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_lde: LDE factor smaller than the number of shards");
-  const u64 L_loc = ctx->shard.local_cosets(L);  // cosets owned by this context (all of them without a shard)
+  if (s && log_n <= s) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_lde: fewer than 2 rows per row block of the domain shard");
+  const u64 w_row = next_row ? gl::omega(log_n) : 1;
+  if (s) {
+    // split shard: per owned unit, fold the monomials onto the row block (straight into the unit's output slot), then one
+    // in-place forward transform of size n / B on the unit's shift
+    const int mb = (int)(log_n - s);
+    const u64 nb = 1ull << mb, U_loc = ctx->shard.local_units(L);
+    u32 chunk = (u32)std::max<u64>(1, std::min<u64>(n_cols, (1ull << 26) / n));
+    const bool two_bufs = !from_monomials && inverse_needs_scratch(ctx, (int)log_n);
+    for (u32 c0 = 0; c0 < n_cols; c0 += chunk) {
+      const u32 cnt = std::min(chunk, n_cols - c0);
+      const u64* mono = (const u64*)d_in + (u64)c0 * in_col_stride;
+      u64 mono_stride = in_col_stride;
+      if (!from_monomials) {
+        BJ_TRY(ensure_scratch(ctx, sizeof(u64) * n * chunk * (two_bufs ? 2 : 1)));
+        u64* mbuf = (u64*)ctx->scratch;
+        BJ_TRY(run_transform(ctx, mono, in_col_stride, mbuf, n, (int)log_n, cnt, 1, true, two_bufs ? mbuf + n * chunk : nullptr, n));
+        mono = mbuf;
+        mono_stride = n;
+      }
+      for (u64 k = 0; k < U_loc; k++) {
+        const u64 sigma = gl::mul(ctx->shard.unit_shift(ctx->shard.global_unit(k), log_n, log_lde), w_row);
+        UnitPowers pw{};
+        const u64 sb = gl::pow(sigma, nb);
+        pw.v[0] = 1;
+        for (u32 i = 1; i < (1u << s); i++) pw.v[i] = gl::mul(pw.v[i - 1], sb);
+        u64* out = (u64*)d_out + ((u64)c0 * U_loc + k) * nb;
+        const u64 total = (u64)cnt << mb;
+        lde_unit_fold_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ctx->stream>>>(mono, mono_stride, out, nb * U_loc, mb, 1u << s, total, pw);
+        BJ_LAUNCH_CHECK(ctx);
+        BJ_TRY(run_transform(ctx, out, nb * U_loc, out, nb * U_loc, mb, cnt, sigma, false, nullptr, 0));
+      }
+    }
+    return BJ_OK;
+  }
+  const u64 L_loc = ctx->shard.local_units(L);  // cosets owned by this context (all of them without a shard)
   const int m = (int)log_n;
   // per chunk of columns: monomials (natural order) in scratch, then one forward transform per coset that
   // reads the monomials and writes straight into the coset's slot of d_out.
   const bool two_bufs = !from_monomials && inverse_needs_scratch(ctx, m);
   u32 chunk = (u32)std::max<u64>(1, std::min<u64>(n_cols, (1ull << 26) / n));
-  const u64 w_big = gl::omega(log_n + log_lde);
   for (u32 c0 = 0; c0 < n_cols; c0 += chunk) {
     const u32 cnt = std::min(chunk, n_cols - c0);
     const u64* in = (const u64*)d_in + (u64)c0 * in_col_stride;
@@ -658,15 +715,29 @@ int32_t bj_lde(bj_ctx* ctx, const uint64_t* d_in, uint64_t in_col_stride, uint64
       mono_stride = n;
     }
     for (u64 k = 0; k < L_loc; k++) {
-      const u64 j = (k << ctx->shard.log_stride) | ctx->shard.first;  // global coset of local slot k
-      u64 jr = 0;
-      for (uint32_t b = 0; b < log_lde; b++) jr |= ((j >> b) & 1) << (log_lde - 1 - b);
-      const u64 shift = gl::mul(gl::MULT_GEN, gl::pow(w_big, jr));
+      u64 shift = ctx->shard.unit_shift(ctx->shard.global_unit(k), log_n, log_lde);  // the coset of local slot k
+      if (next_row) shift = gl::mul(shift, w_row);
       u64* out = (u64*)d_out + ((u64)c0 * L_loc + k) * n;
       BJ_TRY(run_transform(ctx, mono, mono_stride, out, n * L_loc, m, cnt, shift, false, nullptr, 0));
     }
   }
   return BJ_OK;
+}
+
+}  // namespace bj
+
+extern "C" {
+
+int32_t bj_lde(bj_ctx* ctx, const uint64_t* d_in, uint64_t in_col_stride, uint64_t* d_out, uint32_t log_n,
+               uint32_t log_lde, uint32_t n_cols, int32_t from_monomials) {
+  bj::DeviceGuard device_guard(ctx);
+  return lde_impl(ctx, d_in, in_col_stride, d_out, log_n, log_lde, n_cols, from_monomials, false);
+}
+
+int32_t bj_lde_next_row(bj_ctx* ctx, const uint64_t* d_in, uint64_t in_col_stride, uint64_t* d_out, uint32_t log_n,
+                        uint32_t log_lde, uint32_t n_cols, int32_t from_monomials) {
+  bj::DeviceGuard device_guard(ctx);
+  return lde_impl(ctx, d_in, in_col_stride, d_out, log_n, log_lde, n_cols, from_monomials, true);
 }
 
 // Host-buffer entry points: the batch is cut into column chunks that flow through a 3-slot device ring, upload of chunk

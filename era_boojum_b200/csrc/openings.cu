@@ -6,7 +6,9 @@
 // Fp2-valued polynomials are stored as two base columns and are evaluated column by column (f = f0 + u f1).
 // On a coset-sharded context (multi-GPU) local slot 0 is the global coset j = rank with shift c = 7 w_{nL}^{bitrev_L(j)}
 // instead of 7: the same formula with c in place of 7 gives the same f(at), so every rank can open any column from the
-// coset it owns and the columns are split over the ranks.
+// coset it owns and the columns are split over the ranks.  On a split domain shard local slot 0 is one row block of coset
+// j: the sum runs over that block's rows with the whole coset's scale and the result is the block's CONTRIBUTION; the B
+// contributions of the ranks holding coset j add up to f(at).
 #include <vector>
 #include "ctx.hpp"
 
@@ -89,39 +91,38 @@ extern "C" int32_t bj_barycentric_evaluate(bj_ctx* ctx, const uint64_t* const* h
   if (!ctx || !h_cols || !h_at || !h_out || n_cols == 0 || log_n > 32)
     BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_barycentric_evaluate: bad argument");
   const u64 n = 1ull << log_n;
-  // shift of the coset in local slot 0: 7 * w_{nL}^{bitrev_L(first)} (7 itself without a shard / on rank 0)
+  // shift of the unit in local slot 0 (the global unit `first`): 7 * w_{nL}^{bitrev_L(j)} for a whole coset (7 itself without a
+  // shard / on rank 0), times w_n^{bitrev_s(p)} for row block p of a split shard, which sums over its n / B rows only
+  const u32 split = ctx->shard.log_split;
+  if (split >= log_n && split) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_barycentric_evaluate: fewer rows than row blocks of the domain shard");
+  const u64 rows = n >> split;
   u64 shift = gl::MULT_GEN;
-  if (ctx->shard.first) {
-    const u32 ll = ctx->shard_log_lde;
-    u64 jr = 0;
-    for (u32 b = 0; b < ll; b++) jr |= (u64)((ctx->shard.first >> b) & 1) << (ll - 1 - b);
-    shift = gl::mul(gl::MULT_GEN, gl::pow(gl::omega(log_n + ll), jr));
-  }
+  if (ctx->shard.first) shift = ctx->shard.unit_shift(ctx->shard.first, log_n, ctx->shard_log_lde);
   BJ_TRY(ensure_twiddles(ctx, (int)log_n));
   const gl::e2 at = {gl::canon(h_at[0]), gl::canon(h_at[1])};
-  // scale = (at^n - c^n) / (n * c^n), c = shift
+  // scale = (at^n - c^n) / (n * c^n), c = the coset's shift (c^n = shift^n: the row-block factor is an n-th root of unity)
   gl::e2 atn = at;
   for (u32 i = 0; i < log_n; i++) atn = gl::e2_sqr(atn);
   const u64 cn = gl::pow(shift, n);
   gl::e2 scale = {gl::canon(gl::sub(atn.c0, cn)), atn.c1};
   scale = gl::e2_mul_base(scale, gl::inv(gl::mul(gl::canon(n % gl::P), cn)));
-  const u32 gx = (u32)std::min<u64>((n + DOT_T - 1) / DOT_T, 4 * (u64)ctx->sm_count);
-  const size_t need = sizeof(u64) * (3 * n + (size_t)gx * n_cols * 2);
+  const u32 gx = (u32)std::min<u64>((rows + DOT_T - 1) / DOT_T, 4 * (u64)ctx->sm_count);
+  const size_t need = sizeof(u64) * (3 * rows + (size_t)gx * n_cols * 2);
   BJ_TRY(ensure_scratch(ctx, need));
   u64* w0 = (u64*)ctx->scratch;
-  u64* w1 = w0 + n;
-  u64* xs = w1 + n;
-  u64* partial = xs + n;
-  const unsigned blocks = (unsigned)((n + 255) / 256);
-  bary_denominators_kernel<<<blocks, 256, 0, ctx->stream>>>(ctx->tw_fwd, n, at, shift, w0, w1, xs);
+  u64* w1 = w0 + rows;
+  u64* xs = w1 + rows;
+  u64* partial = xs + rows;
+  const unsigned blocks = (unsigned)((rows + 255) / 256);
+  bary_denominators_kernel<<<blocks, 256, 0, ctx->stream>>>(ctx->tw_fwd, rows, at, shift, w0, w1, xs);
   BJ_LAUNCH_CHECK(ctx);
-  BJ_TRY(bj_batch_inverse_ext(ctx, (uint64_t*)w0, (uint64_t*)w1, n));
-  bary_weights_kernel<<<blocks, 256, 0, ctx->stream>>>(w0, w1, xs, n, scale);
+  BJ_TRY(bj_batch_inverse_ext(ctx, (uint64_t*)w0, (uint64_t*)w1, rows));
+  bary_weights_kernel<<<blocks, 256, 0, ctx->stream>>>(w0, w1, xs, rows, scale);
   BJ_LAUNCH_CHECK(ctx);
   void* d;
   BJ_TRY(param_upload(ctx, h_cols, sizeof(u64*) * n_cols, &d));
   dim3 grid(gx, (n_cols + DOT_COLS - 1) / DOT_COLS);
-  bary_dot_kernel<<<grid, DOT_T, 0, ctx->stream>>>((const u64* const*)d, n_cols, n, w0, w1, partial);
+  bary_dot_kernel<<<grid, DOT_T, 0, ctx->stream>>>((const u64* const*)d, n_cols, rows, w0, w1, partial);
   BJ_LAUNCH_CHECK(ctx);
   std::vector<u64> hp((size_t)gx * n_cols * 2);
   BJ_CUDA(ctx, cudaMemcpyAsync(hp.data(), partial, sizeof(u64) * hp.size(), cudaMemcpyDeviceToHost, ctx->stream));

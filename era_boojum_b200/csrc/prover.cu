@@ -253,9 +253,12 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
     BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_setup_create: inconsistent lookup description");
   if (ctx->shard.log_stride && !ctx->comm)
     BJ_FAIL(ctx, BJ_ERR_UNSUPPORTED, "bj_setup_create: a coset-sharded context needs a communicator (bj_comm_create_*) for the native driver");
-  if (ctx->comm && (circuit->merkle_tree_cap_size < circuit->fri_lde_factor || comm_world(ctx) > circuit->fri_lde_factor ||
+  const uint32_t split = ctx->shard.log_split;  // row blocks per coset = 2^split when there are more ranks than cosets
+  if (ctx->comm && (circuit->merkle_tree_cap_size < std::max(circuit->fri_lde_factor, comm_world(ctx)) ||
                     (1u << ctx->shard_log_lde) != circuit->fri_lde_factor))
-    BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_setup_create: sharded proving needs cap_size >= LDE factor >= world and the LDE factor the communicator was created for");
+    BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_setup_create: sharded proving needs cap_size >= max(LDE factor, world) and the LDE factor the communicator was created for");
+  if (ctx->comm && split && circuit->log_n <= split)
+    BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_setup_create: a row block of the domain shard needs at least 2 rows (2^log_n >= 2 * world / LDE factor)");
   *out = nullptr;
   {
     // a proof needs at least one FRI folding step (the JSON has a fri_base_oracle_cap): reject circuits so small that
@@ -268,6 +271,13 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
     if (sched_len == 0)
       BJ_FAIL(ctx, BJ_ERR_INVALID_ARG,
               "bj_setup_create: degenerate instance - 2^log_n * fri_lde_factor is too small for merkle_tree_cap_size (empty FRI schedule)");
+    // a FRI fold stays inside one unit of the shard: every level's units must hold the 2^k elements it folds together
+    uint32_t log_unit = circuit->log_n - (ctx->comm ? split : 0);
+    for (uint32_t i = 0; i < sched_len; i++) {
+      if (log_unit < sched[i])
+        BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_setup_create: a FRI level has fewer elements per unit of the domain shard than it folds together");
+      log_unit -= sched[i];
+    }
   }
   std::unique_ptr<bj_setup> s(new bj_setup());
   s->ctx = ctx;
@@ -343,11 +353,13 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   uint32_t log_q = 0;
   while ((1u << log_q) < Q) log_q++;
   const u64 n = 1ull << log_n, nQ = n << log_q;
-  // coset shard (multi-GPU): this context holds L / world cosets of every LDE column and Q_loc of the first Q cosets
+  // domain shard (multi-GPU): this context holds (L << split) / world units of every LDE column and its units of the first Q cosets
   const uint32_t world = comm_world(ctx), rank = comm_rank(ctx);
   const u64 nL = (n << log_l) / world;                                   // LOCAL length of the committed part of an LDE column
   const u64 nD = (n << log_d) / world;                                   // LOCAL length (= stride) of an LDE column, D = max(L, Q)
-  const u64 nQl = ctx->shard.local_cosets(Q) << log_n;                    // LOCAL quotient points
+  const u64 nQl = ctx->shard.local_points(Q, (int)log_n);                 // LOCAL quotient points
+  const uint32_t split = ctx->shard.log_split;                            // 2^split row blocks per coset (split domain shard)
+  const u64 nb = n >> split;                                             // rows of one unit
   if (setup->col_len != nD) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: the setup was built with a different shard");
   const uint32_t T = setup->n_tables, wdt = c.lookup_width, nsub = c.lookup_num_repetitions, voff = c.lookup_variables_offset;
   auto t_prev = std::chrono::steady_clock::now();
@@ -437,6 +449,13 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   }
   BJ_TRY(s2_lde.alloc(ctx, (size_t)n_s2 * nD));
   BJ_TRY(lde_columns(ctx, (const uint64_t*)st2.p, (uint64_t*)s2_lde.p, log_n, log_d, n_s2));
+  // a row block of a split shard does not hold z(omega x) (another block of the coset does).  On a unit with shift sigma,
+  // z(omega x) is the LDE of z on the shift sigma * omega in the same row order: two more columns (c0, c1 of z)
+  DevMem z_next;
+  if (split && ctx->shard.local_units(Q)) {
+    BJ_TRY(z_next.alloc(ctx, 2 * nD));
+    BJ_TRY(bj_lde_next_row(ctx, (const uint64_t*)st2.p, n, (uint64_t*)z_next.p, log_n, log_d, 2, 0));
+  }
   st2.release();
   std::vector<const uint64_t*> s2_cols(n_s2);
   for (uint32_t j = 0; j < n_s2; j++) s2_cols[j] = (const uint64_t*)s2_lde.p + (size_t)j * nD;
@@ -498,34 +517,41 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     std::vector<uint64_t> nr(V);
     BJ_TRY(bj_non_residues_for_copy_permutation(n, V, nr.data()));
     const uint64_t b[2] = {beta.c0, beta.c1}, g[2] = {gamma.c0, gamma.c1};
-    BJ_TRY(bj_quotient_copy_permutation(ctx, w_cols.data(), sigma_cols.data(), V, nr.data(), s2_cols[0], s2_cols[1],
-                                        n_partial ? s2_cols.data() + 2 : nullptr, b, g, powers.data() + 2 * (size_t)(n_lk_terms + n_gate_terms),
-                                        log_n, log_d, log_q, Q, q0, q1));
+    if (split)
+      BJ_TRY(bj_quotient_copy_permutation_with_z_next(ctx, w_cols.data(), sigma_cols.data(), V, nr.data(), s2_cols[0], s2_cols[1], (const uint64_t*)z_next.p,
+                                                      (const uint64_t*)z_next.p + nD, n_partial ? s2_cols.data() + 2 : nullptr, b, g,
+                                                      powers.data() + 2 * (size_t)(n_lk_terms + n_gate_terms), log_n, log_d, log_q, Q, q0, q1));
+    else
+      BJ_TRY(bj_quotient_copy_permutation(ctx, w_cols.data(), sigma_cols.data(), V, nr.data(), s2_cols[0], s2_cols[1],
+                                          n_partial ? s2_cols.data() + 2 : nullptr, b, g, powers.data() + 2 * (size_t)(n_lk_terms + n_gate_terms),
+                                          log_n, log_d, log_q, Q, q0, q1));
   }
   BJ_TRY(bj_quotient_divide_by_vanishing(ctx, q0, q1, log_n, log_q));
   }  // nQl
+  z_next.release();
   if (world > 1) {
     // the one bulk exchange: the quotient cosets recombine (they are interpolated together at size n * Q).  Every rank sends
-    // `per` = ceil(Q / world) coset slots (c0 | c1 per slot; ranks beyond Q send padding), one all-gather, then the owned
-    // slots are scattered to their global coset positions j = k * world + r.
-    const u64 per = std::max<u64>(1, Q / world);
+    // `per` = ceil(Q * B / world) unit slots of nb = n / B rows (c0 | c1 per slot; ranks beyond the Q * B units send
+    // padding), one all-gather, then the slots are scattered to their global unit positions.
+    const u64 q_units = (u64)Q << split;
+    const u64 per = std::max<u64>(1, q_units / world);
     DevMem snd, rcv;
-    BJ_TRY(snd.alloc(ctx, per * 2 * n));
-    BJ_TRY(rcv.alloc(ctx, (u64)world * per * 2 * n));
-    BJ_CUDA(ctx, cudaMemsetAsync(snd.p, 0, sizeof(u64) * per * 2 * n, ctx->stream));
-    const u64 q_loc = nQl >> log_n;
+    BJ_TRY(snd.alloc(ctx, per * 2 * nb));
+    BJ_TRY(rcv.alloc(ctx, (u64)world * per * 2 * nb));
+    BJ_CUDA(ctx, cudaMemsetAsync(snd.p, 0, sizeof(u64) * per * 2 * nb, ctx->stream));
+    const u64 q_loc = ctx->shard.local_units(Q);
     for (u64 k = 0; k < q_loc; k++) {
-      BJ_CUDA(ctx, cudaMemcpyAsync(snd.p + (2 * k) * n, q0 + k * n, sizeof(u64) * n, cudaMemcpyDeviceToDevice, ctx->stream));
-      BJ_CUDA(ctx, cudaMemcpyAsync(snd.p + (2 * k + 1) * n, q1 + k * n, sizeof(u64) * n, cudaMemcpyDeviceToDevice, ctx->stream));
+      BJ_CUDA(ctx, cudaMemcpyAsync(snd.p + (2 * k) * nb, q0 + k * nb, sizeof(u64) * nb, cudaMemcpyDeviceToDevice, ctx->stream));
+      BJ_CUDA(ctx, cudaMemcpyAsync(snd.p + (2 * k + 1) * nb, q1 + k * nb, sizeof(u64) * nb, cudaMemcpyDeviceToDevice, ctx->stream));
     }
-    BJ_TRY(comm_all_gather(ctx->comm, snd.p, rcv.p, per * 2 * n));
+    BJ_TRY(comm_all_gather(ctx->comm, snd.p, rcv.p, per * 2 * nb));
     for (uint32_t r = 0; r < world; r++)
       for (u64 k = 0; k < per; k++) {
-        const u64 j = k * world + r;
-        if (j >= Q) continue;
-        const u64* part = rcv.p + ((u64)r * per + k) * 2 * n;
-        BJ_CUDA(ctx, cudaMemcpyAsync(gq0 + j * n, part, sizeof(u64) * n, cudaMemcpyDeviceToDevice, ctx->stream));
-        BJ_CUDA(ctx, cudaMemcpyAsync(gq1 + j * n, part + n, sizeof(u64) * n, cudaMemcpyDeviceToDevice, ctx->stream));
+        const u64 u = ctx->shard.unit_of(r, k);
+        if (u >= q_units) continue;
+        const u64* part = rcv.p + ((u64)r * per + k) * 2 * nb;
+        BJ_CUDA(ctx, cudaMemcpyAsync(gq0 + u * nb, part, sizeof(u64) * nb, cudaMemcpyDeviceToDevice, ctx->stream));
+        BJ_CUDA(ctx, cudaMemcpyAsync(gq1 + u * nb, part + nb, sizeof(u64) * nb, cudaMemcpyDeviceToDevice, ctx->stream));
       }
     q0 = gq0;
     q1 = gq1;
@@ -597,13 +623,21 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     if (world == 1) {
       BJ_TRY(bj_barycentric_evaluate(ctx, flat.data(), (uint32_t)flat.size(), log_n, a, ev.data()));
     } else {
-      // the columns are split over the ranks (every rank opens its block from the coset it owns), results are gathered
-      const size_t per = (flat.size() + world - 1) / world, first = std::min(flat.size(), (size_t)rank * per);
+      // the columns are split over the coset groups: ranks [g B, (g + 1) B) hold the B row blocks of coset g (B = 1: one rank,
+      // its whole coset) and open column block g from it, each rank its block's contribution.  The contributions are
+      // gathered and the B of a group summed.
+      const uint32_t groups = world >> split, g = rank >> split;
+      const size_t per = (flat.size() + groups - 1) / groups, first = std::min(flat.size(), (size_t)g * per);
       const size_t cnt = std::min(per, flat.size() - first);
       std::vector<uint64_t> mine(2 * per, 0), all(2 * per * world);
       if (cnt) BJ_TRY(bj_barycentric_evaluate(ctx, flat.data() + first, (uint32_t)cnt, log_n, a, mine.data()));
       BJ_TRY(comm_all_gather_host(ctx->comm, (const u64*)mine.data(), (u64*)all.data(), 2 * per));
-      memcpy(ev.data(), all.data(), sizeof(uint64_t) * ev.size());   // rank blocks are contiguous: [r][per] == flat order
+      for (uint32_t gg = 0; gg < groups; gg++)
+        for (size_t e = 0; e < 2 * per && gg * 2 * per + e < ev.size(); e++) {
+          u64 v = 0;
+          for (uint32_t p = 0; p < (1u << split); p++) v = gl::canon(gl::add(v, all[(((size_t)gg << split) + p) * 2 * per + e]));
+          ev[gg * 2 * per + e] = v;   // group blocks are contiguous: [g][per] == flat order
+        }
     }
     size_t k = 0;
     for (const auto& s : srcs) {
@@ -725,14 +759,13 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   std::vector<uint64_t> idxs(num_queries);
   for (auto& i : idxs) i = bj_transcript_get_index_bits(tr, max_bits, max_bits);
   pf->queries.assign(num_queries, {});
-  // a query is answered by the rank that owns the coset of its index (leaf t = coset * n + row lies in that rank's subtree);
+  // a query is answered by the rank that owns the unit of its index (leaf t = coset * n + row lies in that rank's subtree);
   // the other ranks look up a dummy leaf, the answers are exchanged and every rank keeps the owner's
   std::vector<uint64_t> loc_idx(num_queries);
   std::vector<uint32_t> owner(num_queries);
   for (uint32_t q = 0; q < num_queries; q++) {
-    const uint64_t j = idxs[q] >> log_n, i = idxs[q] & (n - 1);
-    owner[q] = (uint32_t)(j % world);
-    loc_idx[q] = owner[q] == rank ? (((j / world) << log_n) | i) : 0;
+    owner[q] = ctx->shard.owner(idxs[q], (int)log_n);
+    loc_idx[q] = owner[q] == rank ? ctx->shard.owner_index(idxs[q], (int)log_n) : 0;
   }
   // every answer part (leaf elements / path of one oracle) is gathered locally first; ONE exchange then carries all of them
   struct Part {
@@ -762,8 +795,7 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
       const size_t le_len = (size_t)2 << k;
       std::vector<uint64_t> locals(num_queries);
       for (uint32_t q = 0; q < num_queries; q++) {
-        const uint64_t j = sub[q] >> log_len, i = sub[q] & ((1ull << log_len) - 1);
-        locals[q] = owner[q] == rank ? ((((j / world) << log_len) | i) >> k) : 0;
+        locals[q] = owner[q] == rank ? (ctx->shard.owner_index(sub[q], (int)log_len) >> k) : 0;
         sub[q] >>= k;
       }
       uint32_t plen = 0;

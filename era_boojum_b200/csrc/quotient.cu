@@ -20,6 +20,8 @@ struct QCopyPermParams {
   u32 n_cols, chunk, n_chunks;
   const u64* z_c0;
   const u64* z_c1;
+  const u64* z_next_c0;        // z(omega x) on the same points (split domain shard), or nullptr: read z at bitrev(bitrev(i) + 1)
+  const u64* z_next_c1;
   const u64* const* partials;  // 2 * (n_chunks - 1) pointers: c0, c1 of each partial product LDE
   gl::e2 beta, gamma;
   const u64* alphas;           // (n_chunks + 1) Fp2: z(1)=1 term first, then one per relation
@@ -32,6 +34,7 @@ struct QCopyPermParams {
   u64* q_c1;
 };
 
+template <bool kZNext>
 __global__ void __launch_bounds__(128) quotient_copy_perm_kernel(const QCopyPermParams p) {
   const u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= p.n_points) return;
@@ -48,9 +51,10 @@ __global__ void __launch_bounds__(128) quotient_copy_perm_kernel(const QCopyPerm
     gl::e2 v = {gl::mul(gl::sub(z.c0, 1), l1), gl::mul(z.c1, l1)};
     q = gl::e2_mul(v, {__ldg(p.alphas), __ldg(p.alphas + 1)});
   }
-  // z(omega x): same coset, position bitrev(bitrev(i) + 1)
+  // z(omega x): same coset, position bitrev(bitrev(i) + 1); a row block of a split shard does not hold that row, so there
+  // z(omega x) comes as its own LDE columns
   u64 ish = 0;
-  if (p.log_n) {
+  if (!kZNext && p.log_n) {
     const u64 nat = (__brevll(i) >> (64 - p.log_n)) + 1;
     ish = __brevll(nat & (n - 1)) >> (64 - p.log_n);
   }
@@ -60,6 +64,7 @@ __global__ void __launch_bounds__(128) quotient_copy_perm_kernel(const QCopyPerm
   for (u32 c = 0; c < p.n_chunks; c++) {
     gl::e2 lhs, rhs;
     if (c + 1 < p.n_chunks) lhs = {p.partials[2 * c][t], p.partials[2 * c + 1][t]};
+    else if (kZNext) lhs = {p.z_next_c0[t], p.z_next_c1[t]};
     else lhs = {p.z_c0[tsh], p.z_c1[tsh]};
     if (c == 0) rhs = z;
     else rhs = {p.partials[2 * (c - 1)][t], p.partials[2 * (c - 1) + 1][t]};
@@ -114,21 +119,18 @@ static void coset_vanishing_values(u32 log_n, u32 log_q, std::vector<u64>& out) 
   }
 }
 
-}  // namespace bj
-
-using namespace bj;
-
-extern "C" {
-
-int32_t bj_quotient_copy_permutation(bj_ctx* ctx, const uint64_t* const* h_variable_ldes, const uint64_t* const* h_sigma_ldes,
-                                     uint32_t n_cols, const uint64_t* h_non_residues, const uint64_t* d_z_c0,
-                                     const uint64_t* d_z_c1, const uint64_t* const* h_partial_ldes, const uint64_t h_beta[2],
-                                     const uint64_t h_gamma[2], const uint64_t* h_alphas, uint32_t log_n, uint32_t log_lde,
-                                     uint32_t log_quotient_degree, uint32_t chunk_size, uint64_t* d_q_c0, uint64_t* d_q_c1) {
-  bj::DeviceGuard device_guard(ctx);
+static int32_t quotient_copy_permutation(bj_ctx* ctx, const uint64_t* const* h_variable_ldes, const uint64_t* const* h_sigma_ldes,
+                                         uint32_t n_cols, const uint64_t* h_non_residues, const uint64_t* d_z_c0, const uint64_t* d_z_c1,
+                                         const uint64_t* d_z_next_c0, const uint64_t* d_z_next_c1, const uint64_t* const* h_partial_ldes,
+                                         const uint64_t h_beta[2], const uint64_t h_gamma[2], const uint64_t* h_alphas, uint32_t log_n,
+                                         uint32_t log_lde, uint32_t log_quotient_degree, uint32_t chunk_size, uint64_t* d_q_c0, uint64_t* d_q_c1) {
   if (!ctx || !h_variable_ldes || !h_sigma_ldes || !h_non_residues || !d_z_c0 || !d_z_c1 || !h_beta || !h_gamma || !h_alphas ||
       !d_q_c0 || !d_q_c1 || n_cols == 0 || chunk_size == 0 || log_quotient_degree > log_lde || log_n + log_lde > 32)
     BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_quotient_copy_permutation: bad argument");
+  if (!d_z_next_c0 != !d_z_next_c1) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_quotient_copy_permutation: z(omega x) needs both components");
+  if (ctx->shard.log_split && !d_z_next_c0)
+    BJ_FAIL(ctx, BJ_ERR_UNSUPPORTED,
+            "bj_quotient_copy_permutation: a row block of a split domain shard does not hold z(omega x) - use bj_quotient_copy_permutation_with_z_next");
   const u32 n_chunks = (n_cols + chunk_size - 1) / chunk_size;
   if (n_chunks > 1 && !h_partial_ldes) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_quotient_copy_permutation: partial products missing");
   BJ_TRY(ensure_twiddles(ctx, (int)(log_n + log_lde)));
@@ -159,18 +161,50 @@ int32_t bj_quotient_copy_permutation(bj_ctx* ctx, const uint64_t* const* h_varia
   p.n_chunks = n_chunks;
   p.z_c0 = (const u64*)d_z_c0;
   p.z_c1 = (const u64*)d_z_c1;
+  p.z_next_c0 = (const u64*)d_z_next_c0;
+  p.z_next_c1 = (const u64*)d_z_next_c1;
   p.beta = {gl::canon(h_beta[0]), gl::canon(h_beta[1])};
   p.gamma = {gl::canon(h_gamma[0]), gl::canon(h_gamma[1])};
   p.tab = ctx->tw_fwd;
   p.log_n = (int)log_n;
   p.shard = ctx->shard;
-  p.n_points = ctx->shard.local_cosets(1ull << log_quotient_degree) << log_n;
+  p.n_points = ctx->shard.local_points(1ull << log_quotient_degree, (int)log_n);
   if (p.n_points == 0) return BJ_OK;  // this shard owns none of the quotient cosets
   p.q_c0 = (u64*)d_q_c0;
   p.q_c1 = (u64*)d_q_c1;
-  quotient_copy_perm_kernel<<<(unsigned)((p.n_points + 127) / 128), 128, 0, ctx->stream>>>(p);
+  if (d_z_next_c0) quotient_copy_perm_kernel<true><<<(unsigned)((p.n_points + 127) / 128), 128, 0, ctx->stream>>>(p);
+  else quotient_copy_perm_kernel<false><<<(unsigned)((p.n_points + 127) / 128), 128, 0, ctx->stream>>>(p);
   BJ_LAUNCH_CHECK(ctx);
   return BJ_OK;
+}
+
+}  // namespace bj
+
+using namespace bj;
+
+extern "C" {
+
+int32_t bj_quotient_copy_permutation(bj_ctx* ctx, const uint64_t* const* h_variable_ldes, const uint64_t* const* h_sigma_ldes,
+                                     uint32_t n_cols, const uint64_t* h_non_residues, const uint64_t* d_z_c0,
+                                     const uint64_t* d_z_c1, const uint64_t* const* h_partial_ldes, const uint64_t h_beta[2],
+                                     const uint64_t h_gamma[2], const uint64_t* h_alphas, uint32_t log_n, uint32_t log_lde,
+                                     uint32_t log_quotient_degree, uint32_t chunk_size, uint64_t* d_q_c0, uint64_t* d_q_c1) {
+  bj::DeviceGuard device_guard(ctx);
+  return quotient_copy_permutation(ctx, h_variable_ldes, h_sigma_ldes, n_cols, h_non_residues, d_z_c0, d_z_c1, nullptr, nullptr,
+                                   h_partial_ldes, h_beta, h_gamma, h_alphas, log_n, log_lde, log_quotient_degree, chunk_size, d_q_c0, d_q_c1);
+}
+
+int32_t bj_quotient_copy_permutation_with_z_next(bj_ctx* ctx, const uint64_t* const* h_variable_ldes, const uint64_t* const* h_sigma_ldes,
+                                                 uint32_t n_cols, const uint64_t* h_non_residues, const uint64_t* d_z_c0,
+                                                 const uint64_t* d_z_c1, const uint64_t* d_z_next_c0, const uint64_t* d_z_next_c1,
+                                                 const uint64_t* const* h_partial_ldes, const uint64_t h_beta[2], const uint64_t h_gamma[2],
+                                                 const uint64_t* h_alphas, uint32_t log_n, uint32_t log_lde, uint32_t log_quotient_degree,
+                                                 uint32_t chunk_size, uint64_t* d_q_c0, uint64_t* d_q_c1) {
+  bj::DeviceGuard device_guard(ctx);
+  if (ctx && (!d_z_next_c0 || !d_z_next_c1))
+    BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_quotient_copy_permutation_with_z_next: z(omega x) columns missing");
+  return quotient_copy_permutation(ctx, h_variable_ldes, h_sigma_ldes, n_cols, h_non_residues, d_z_c0, d_z_c1, d_z_next_c0, d_z_next_c1,
+                                   h_partial_ldes, h_beta, h_gamma, h_alphas, log_n, log_lde, log_quotient_degree, chunk_size, d_q_c0, d_q_c1);
 }
 
 int32_t bj_quotient_divide_by_vanishing(bj_ctx* ctx, uint64_t* d_q_c0, uint64_t* d_q_c1, uint32_t log_n,
@@ -183,7 +217,7 @@ int32_t bj_quotient_divide_by_vanishing(bj_ctx* ctx, uint64_t* d_q_c0, uint64_t*
   for (auto& v : van) v = gl::inv(v);
   void* d;
   BJ_TRY(param_upload(ctx, van.data(), sizeof(u64) * van.size(), &d));
-  const u64 n_points = ctx->shard.local_cosets(1ull << log_quotient_degree) << log_n;
+  const u64 n_points = ctx->shard.local_points(1ull << log_quotient_degree, (int)log_n);
   if (n_points == 0) return BJ_OK;
   scale_by_coset_constant_kernel<<<(unsigned)((n_points + 255) / 256), 256, 0, ctx->stream>>>((u64*)d_q_c0, (u64*)d_q_c1, (int)log_n, n_points,
                                                                                               (const u64*)d, ctx->shard);

@@ -45,6 +45,7 @@ SIGNATURES = {
     "bj_ctx_destroy": (_i32, [_vp]),
     "bj_ctx_set_stream": (_i32, [_vp, _vp]),
     "bj_ctx_set_coset_shard": (_i32, [_vp, _u32, _u32, _u32]),
+    "bj_ctx_set_domain_shard": (_i32, [_vp, _u32, _u32, _u32]),
     "bj_ctx_synchronize": (_i32, [_vp]),
     "bj_last_error": (ctypes.c_char_p, [_vp]),
     "bj_launch_count": (_u64, [_vp]),
@@ -59,6 +60,7 @@ SIGNATURES = {
     "bj_intt_natural_to_natural": (_i32, [_vp, _vp, _u32, _u32, _u64, _u64]),
     "bj_bitreverse": (_i32, [_vp, _vp, _u32, _u32, _u64]),
     "bj_lde": (_i32, [_vp, _vp, _u64, _vp, _u32, _u32, _u32, _i32]),
+    "bj_lde_next_row": (_i32, [_vp, _vp, _u64, _vp, _u32, _u32, _u32, _i32]),
     "bj_merkle_build_poseidon2": (_i32, [_vp, _vp, _u32, _u64, _u32, _u32, _vp, _vp]),
     "bj_merkle_build_blake2s": (_i32, [_vp, _vp, _u32, _u64, _u32, _u32, _vp, _vp]),
     "bj_merkle_build_keccak256": (_i32, [_vp, _vp, _u32, _u64, _u32, _u32, _vp, _vp]),
@@ -71,6 +73,7 @@ SIGNATURES = {
     "bj_non_residues_for_copy_permutation": (_i32, [_u64, _u32, _vp]),
     "bj_copy_permutation_stage2": (_i32, [_vp, _vp, _vp, _u32, _vp, _vp, _vp, _u32, _u32, _vp, _vp, _vp]),
     "bj_quotient_copy_permutation": (_i32, [_vp, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _u32, _u32, _vp, _vp]),
+    "bj_quotient_copy_permutation_with_z_next": (_i32, [_vp, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _u32, _u32, _vp, _vp]),
     "bj_quotient_divide_by_vanishing": (_i32, [_vp, _vp, _vp, _u32, _u32]),
     "bj_barycentric_evaluate": (_i32, [_vp, _vp, _u32, _u32, _vp, _vp]),
     "bj_lookup_polys_specialized": (_i32, [_vp, _vp, _u32, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _u32, _vp]),

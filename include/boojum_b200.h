@@ -64,18 +64,30 @@ BJ_API int32_t bj_ctx_synchronize(bj_ctx* ctx);
  * uses that coset's shift, so any rank can open any column - the same value comes out.
  * The reference has no counterpart (its Worker is one machine's thread pool).  Default: rank 0 of 1. */
 BJ_API int32_t bj_ctx_set_coset_shard(bj_ctx* ctx, uint32_t rank, uint32_t world, uint32_t log_lde);
+/* Domain shard: bj_ctx_set_coset_shard for world <= 2^log_lde.  Above it (world a power of two <= 8 * 2^log_lde) every coset
+ * is cut into B = world / 2^log_lde row blocks: the domain is made of UNITS u = j * B + p, unit u being rows
+ * [p n / B, (p + 1) n / B) of coset j in its bit-reversed row order (flat index t = u * (n / B) + i'), and this context holds
+ * the units u = rank (mod world), stored [local unit][n / B rows].  Row block p of coset j is the coset
+ * sigma * <w_{n/B}> with sigma = 7 w_{nL}^{bitrev_L(j)} w_n^{bitrev_s(p)} (B = 2^s), rows bit-reversed.  Every entry point
+ * that works on a coset shard works on units the same way, with two exceptions: bj_barycentric_evaluate returns the
+ * CONTRIBUTION of the local row block (the B contributions of the ranks that hold coset j add up to the value), and
+ * bj_quotient_copy_permutation, which would read z(omega x) from another row block, returns BJ_ERR_UNSUPPORTED -
+ * bj_quotient_copy_permutation_with_z_next takes z(omega x) as columns (bj_lde_next_row) instead. */
+BJ_API int32_t bj_ctx_set_domain_shard(bj_ctx* ctx, uint32_t rank, uint32_t world, uint32_t log_lde);
 BJ_API const char* bj_last_error(const bj_ctx* ctx);
 /* number of kernels this library launched through ctx so far (for launch accounting) */
 BJ_API uint64_t bj_launch_count(const bj_ctx* ctx);
 
-/* ---- multi-GPU: communicator of the coset-sharded prover (one process - or one thread - per GPU) ----
- * Creating a communicator on a context declares its coset shard (bj_ctx_set_coset_shard(ctx, rank, world, log_lde)) and makes
+/* ---- multi-GPU: communicator of the sharded prover (one process - or one thread - per GPU) ----
+ * Creating a communicator on a context declares its domain shard (bj_ctx_set_domain_shard(ctx, rank, world, log_lde)) and makes
  * bj_setup_create / bj_prove / bj_do_fri on that context run SHARDED: every rank passes the same full witness, keeps the LDE
- * cosets j = rank (mod world) of every committed polynomial, builds the Merkle subtrees of its cosets, and all ranks return
- * the same proof (identical to the single-GPU proof).  What crosses GPUs: cap digests of every oracle, the quotient cosets
- * (one all-gather of 2 * Q * n u64 - they are interpolated together, prover.rs:1399-1467), the openings (computed by the owner
- * of coset 0), the last FRI codeword and the query answers.  Requirements: world a power of two <= the LDE factor,
- * merkle_tree_cap_size >= the LDE factor.
+ * units u = rank (mod world) of every committed polynomial (whole cosets for world <= the LDE factor, row blocks of cosets
+ * above it), builds the Merkle subtrees of its units, and all ranks return the same proof (identical to the single-GPU
+ * proof).  What crosses GPUs: cap digests of every oracle, the quotient units (one all-gather of 2 * Q * n u64 - they are
+ * interpolated together, prover.rs:1399-1467), the openings (each column block opened by one coset group, row-block
+ * contributions summed on the host), the last FRI codeword and the query answers.  Requirements: world a power of two
+ * <= 8 * the LDE factor, merkle_tree_cap_size >= max(LDE factor, world); with row blocks, 2^log_n >= 2 * world / LDE factor
+ * and every FRI level must keep at least the 2^k elements it folds together in each unit.
  *   NCCL transport: rank 0 calls bj_comm_unique_id and hands the 128 bytes to the other ranks by any side channel (MPI, TCP,
  *   torch.distributed ...); every rank then calls bj_comm_create_nccl.  libnccl.so.2 is loaded at run time (the copy already
  *   in the process is reused); BJ_ERR_UNSUPPORTED if it is absent.
@@ -134,6 +146,10 @@ BJ_API int32_t bj_bitreverse(bj_ctx* ctx, uint64_t* d_data, uint32_t log_n, uint
  *        src/cs/implementations/polynomial/lde.rs:161-170).  Column c starts at d_out + c * (n << log_lde). */
 BJ_API int32_t bj_lde(bj_ctx* ctx, const uint64_t* d_in, uint64_t in_col_stride, uint64_t* d_out, uint32_t log_n,
                uint32_t log_lde, uint32_t n_cols, int32_t from_monomials);
+/* bj_lde of g(x) = f(w_n x), same layout: the value at a point is f at the next row's point.  A row block of a split domain
+ * shard reads z(omega x) of the copy-permutation quotient from here (the row itself lives in another block). */
+BJ_API int32_t bj_lde_next_row(bj_ctx* ctx, const uint64_t* d_in, uint64_t in_col_stride, uint64_t* d_out, uint32_t log_n,
+                               uint32_t log_lde, uint32_t n_cols, int32_t from_monomials);
 
 /* ---- Poseidon2 Merkle tree: MerkleTreeWithCap::construct / construct_by_chunking /
  *      construct_by_chunking_from_flat_sources / continue_from_leaf_hashes (src/cs/oracle/merkle_tree.rs:78-449)
@@ -300,6 +316,14 @@ BJ_API int32_t bj_quotient_copy_permutation(bj_ctx* ctx, const uint64_t* const* 
                                      const uint64_t* d_z_c1, const uint64_t* const* h_partial_ldes, const uint64_t h_beta[2],
                                      const uint64_t h_gamma[2], const uint64_t* h_alphas, uint32_t log_n, uint32_t log_lde,
                                      uint32_t log_quotient_degree, uint32_t chunk_size, uint64_t* d_q_c0, uint64_t* d_q_c1);
+/* the same with z(omega x) given as LDE columns (bj_lde_next_row of z) instead of read from z's next row: what a split domain
+ * shard uses, where bj_quotient_copy_permutation returns BJ_ERR_UNSUPPORTED */
+BJ_API int32_t bj_quotient_copy_permutation_with_z_next(bj_ctx* ctx, const uint64_t* const* h_variable_ldes, const uint64_t* const* h_sigma_ldes,
+                                                        uint32_t n_cols, const uint64_t* h_non_residues, const uint64_t* d_z_c0,
+                                                        const uint64_t* d_z_c1, const uint64_t* d_z_next_c0, const uint64_t* d_z_next_c1,
+                                                        const uint64_t* const* h_partial_ldes, const uint64_t h_beta[2], const uint64_t h_gamma[2],
+                                                        const uint64_t* h_alphas, uint32_t log_n, uint32_t log_lde, uint32_t log_quotient_degree,
+                                                        uint32_t chunk_size, uint64_t* d_q_c0, uint64_t* d_q_c1);
 /* divide_by_vanishing_for_bitreversed_coset_enumeration (src/cs/implementations/utils.rs:770-817): q[coset j] *= 1/((7 w^bitrev(j))^n - 1) */
 BJ_API int32_t bj_quotient_divide_by_vanishing(bj_ctx* ctx, uint64_t* d_q_c0, uint64_t* d_q_c1, uint32_t log_n,
                                         uint32_t log_quotient_degree);
@@ -308,6 +332,8 @@ BJ_API int32_t bj_quotient_divide_by_vanishing(bj_ctx* ctx, uint64_t* d_q_c0, ui
  *      (barycentric evaluation, src/cs/implementations/utils.rs:907-1243; prover.rs:1519-1802).
  * h_cols: host array of device pointers to LDE columns (only the first 2^log_n values, coset 0, are read).
  * h_out: n_cols (c0, c1) pairs.  `at` must not lie on the coset 7<w_n> (on a sharded context: on the coset of local slot 0).
+ * On a split domain shard (bj_ctx_set_domain_shard with world > the LDE factor) local slot 0 is one row block of a coset and
+ * h_out is that block's CONTRIBUTION: summing the outputs of the ranks that hold the coset's blocks gives the values.
  * Synchronises. */
 BJ_API int32_t bj_barycentric_evaluate(bj_ctx* ctx, const uint64_t* const* h_cols, uint32_t n_cols, uint32_t log_n,
                                 const uint64_t h_at[2], uint64_t* h_out);

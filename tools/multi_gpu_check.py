@@ -1,6 +1,8 @@
 """torchrun check on N GPUs: column-sharded iNTT -> NCCL all-gather of monomials -> coset-sharded LDE + Merkle subtrees
 -> all-gather of caps equals the single-GPU commitment (bit-exact), plus timings; then the coset-sharded prover
-(prover.prove with a TorchDistComm) must return the single-GPU proof on every rank.  Usage:
+(prover.prove with a TorchDistComm) must return the single-GPU proof on every rank, and so must the library's driver
+(bj_prove over NCCL) on the SHA-bench shape and on the production shape (LDE factor 2: cosets split into row blocks above
+2 ranks).  The first parts use LDE factor 8 and so need N <= 8.  Usage:
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port 29511 tools/multi_gpu_check.py"""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -97,4 +99,27 @@ for hasher, transcript in (("poseidon2", "poseidon"), ("blake2s", "blake2s")):
                "stages_s": {k: round(v, 4) for k, v in tm.items()}})
     nat.close()
 comm.close()
+
+# ---- the production shape (LDE factor 2, quotient degree 8, cap 32) through bj_prove over NCCL: with more ranks than its
+#      2 cosets every coset is split into world / 2 row blocks (up to 16 ranks) ----
+prod_log_n = int(os.environ.get("PROD_LOG_N", "14"))
+pctx = bj.Context.on_current_stream(local)
+pcomm = bj.Comm.from_torch_distributed(pctx, dist, 2)
+pc = synthetic.generate_production_shaped(ctx, prod_log_n, seed=5)
+pcfg = prover.ProofConfig(fri_lde_factor=2, merkle_tree_cap_size=32, security_level=100)
+m = pc["lookup"]["multiplicities"]
+ref = ctx.native_setup(pc["sigmas"], pc["constants"], pc["gates"], 8, pcfg, lookup=pc["lookup"], public_inputs=pc["public_inputs"])
+want = ref.prove(pc["variables"], m)
+ref_cap = ref.get_cap()
+ref.close()
+nat = pctx.native_setup(pc["sigmas"], pc["constants"], pc["gates"], 8, pcfg, lookup=pc["lookup"], public_inputs=pc["public_inputs"])
+got = nat.prove(pc["variables"], m)
+same = json.dumps(want, sort_keys=True) == json.dumps(got, sort_keys=True) and np.array_equal(ref_cap, nat.get_cap())
+flag = torch.tensor([1 if same else 0], device="cuda:%d" % local)
+dist.all_reduce(flag, op=dist.ReduceOp.MIN)
+if rank == 0:
+    print({"world": world, "production_shaped_log_n": prod_log_n, "row_blocks_per_coset": max(1, world // 2),
+           "equals_single_gpu_proof_on_every_rank": bool(flag.item()), "oracle_verifier_accepts": bool(OV.verify(nat.vk(), got))})
+nat.close()
+pcomm.close()
 dist.destroy_process_group()
