@@ -240,6 +240,18 @@ class Context:
     def launch_count(self):
         return int(lib.bj_launch_count(self._h))
 
+    def set_memory_limit(self, nbytes):
+        """bj_ctx_set_memory_limit: device bytes a proof on this context may use (0: what is free when the setup is created).
+        native_setup picks the resident plan if it fits, the compact one otherwise, and raises BoojumError (out of device
+        memory, with both plans' byte counts) if neither does."""
+        self._check(lib.bj_ctx_set_memory_limit(self._h, int(nbytes)))
+
+    def memory_high_water(self, reset=False):
+        """bj_ctx_memory_high_water: the highest device memory the context's pool has had in use (bytes)"""
+        v = ctypes.c_uint64()
+        self._check(lib.bj_ctx_memory_high_water(self._h, ctypes.byref(v), int(bool(reset))))
+        return int(v.value)
+
     @staticmethod
     def _ptr(t):
         return ctypes.c_void_p(t.data_ptr())
@@ -635,6 +647,20 @@ class Comm:
             pass
 
 
+def proof_memory_plan(log_n, num_variables, num_constants, quotient_degree, config, lookup=None, world=1):
+    """bj_proof_memory_plan: device bytes of native_setup + prove at their peak on each of `world` GPUs, counted from the
+    shapes (no device needed).  -> dict(resident=bytes, compact=bytes or None when the compact plan does not apply)."""
+    c = native.Circuit()
+    c.log_n, c.num_variables, c.num_constants, c.quotient_degree = log_n, num_variables, num_constants, quotient_degree
+    c.fri_lde_factor, c.merkle_tree_cap_size = config.fri_lde_factor, config.merkle_tree_cap_size
+    c.security_level, c.pow_bits = config.security_level, config.pow_bits
+    if lookup:
+        c.lookup_width, c.lookup_num_repetitions = lookup["width"], lookup["num_repetitions"]
+    out = (ctypes.c_uint64 * 2)()
+    _ok(lib.bj_proof_memory_plan(ctypes.byref(c), world, out), "bj_proof_memory_plan")
+    return {"resident": int(out[0]), "compact": int(out[1]) or None}
+
+
 class NativeSetup:
     """bj_setup: setup LDE + setup tree + circuit description held by the library; prove() runs bj_prove (host C++)."""
 
@@ -666,6 +692,18 @@ class NativeSetup:
                                        ctx._ptr(lookup["tables"]) if lookup else None, ctypes.byref(h)))
         self._h = h
         del keep
+
+    @property
+    def compact(self):
+        """True if bj_setup_create chose the compact memory plan"""
+        return lib.bj_setup_is_compact(self._h) == 1
+
+    def memory_plan(self):
+        """bj_setup_memory_plan: the chosen plan -> dict(pool=peak pool bytes of setup + prove, outside_pool=bound on the
+        library's other device memory, chunk=columns the compact plan recomputes at a time, 0 on the resident plan)"""
+        out = (ctypes.c_uint64 * 3)()
+        _ok(lib.bj_setup_memory_plan(self._h, out), "bj_setup_memory_plan")
+        return {"pool": int(out[0]), "outside_pool": int(out[1]), "chunk": int(out[2])}
 
     def get_cap(self):
         out = np.zeros((self.cap_size, 4), np.uint64)

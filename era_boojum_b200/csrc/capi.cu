@@ -235,6 +235,27 @@ int32_t bj_ctx_synchronize(bj_ctx* ctx) {
   return BJ_OK;
 }
 
+int32_t bj_ctx_set_memory_limit(bj_ctx* ctx, uint64_t bytes) {
+  if (!ctx) return BJ_ERR_INVALID_ARG;
+  ctx->memory_limit = bytes;
+  return BJ_OK;
+}
+
+int32_t bj_ctx_memory_high_water(bj_ctx* ctx, uint64_t* bytes, int32_t reset) {
+  bj::DeviceGuard device_guard(ctx);
+  if (!ctx || !bytes) return BJ_ERR_INVALID_ARG;
+  if (!ctx->pool) BJ_FAIL(ctx, BJ_ERR_UNSUPPORTED, "bj_ctx_memory_high_water: the context has no memory pool");
+  BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  uint64_t v = 0;
+  BJ_CUDA(ctx, cudaMemPoolGetAttribute(ctx->pool, cudaMemPoolAttrUsedMemHigh, &v));
+  *bytes = v;
+  if (reset) {
+    uint64_t zero = 0;  // the attribute can only be reset to 0: the high-water mark restarts from the current use
+    BJ_CUDA(ctx, cudaMemPoolSetAttribute(ctx->pool, cudaMemPoolAttrUsedMemHigh, &zero));
+  }
+  return BJ_OK;
+}
+
 const char* bj_last_error(const bj_ctx* ctx) { return ctx ? ctx->last_error.c_str() : "no context"; }
 uint64_t bj_launch_count(const bj_ctx* ctx) { return ctx ? ctx->launches : 0; }
 

@@ -123,6 +123,7 @@ struct bj_ctx {
   cudaMemPool_t pool = nullptr;  // private stream-ordered pool of the prover driver (keeps freed blocks: no OS round trips per proof)
   bj::CosetShard shard;  // bj_ctx_set_coset_shard / bj_ctx_set_domain_shard; default = the whole domain
   uint32_t shard_log_lde = 0;  // LDE factor the shard was declared for (locates the coset bits of flat indices)
+  uint64_t memory_limit = 0;   // bj_ctx_set_memory_limit: device bytes a proof may use (0: what is free when the setup is created)
 };
 
 #define BJ_FAIL(ctx, code, msg)          \

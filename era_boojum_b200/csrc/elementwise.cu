@@ -121,6 +121,7 @@ struct DeepParams {
   gl::e2 k_const;            // sum_i ch_i * value_at_i  (precomputed on the host)
   u64* acc_c0;
   u64* acc_c1;
+  u64 first;                 // RANGE kernel: global index of point 0 (the buffers hold points [first, first + n_rows))
 };
 
 // Unreduced accumulator for sums of 64x64-bit products: 128 bits + an overflow word (exact for < 2^32 terms).  One
@@ -141,6 +142,9 @@ __device__ __forceinline__ u64 acc_reduce(const Acc160& a) {
 
 constexpr int DEEP_U = 4;  // columns whose loads are issued together (memory-level parallelism: the kernel streams ~70 GB)
 
+// RANGE = false: the whole domain of this context (x(t) through the shard's global index).  RANGE = true: an unsharded run of
+// n_rows consecutive points starting at the global index p.first (a few cosets of the domain, e.g. one recomputed coset).
+template <bool RANGE>
 __global__ void __launch_bounds__(256) deep_group_kernel(const DeepParams p) {
   const u64 stride = (u64)gridDim.x * blockDim.x;
   const u64 t0 = (u64)blockIdx.x * blockDim.x + threadIdx.x;
@@ -194,7 +198,7 @@ __global__ void __launch_bounds__(256) deep_group_kernel(const DeepParams p) {
     const u64 t = t0 + r * stride;
     pre[r] = acc;
     if (t < p.n_rows) {
-      const u64 tg = p.shard.global_index(t, p.log_n);
+      const u64 tg = RANGE ? p.first + t : p.shard.global_index(t, p.log_n);
       u64 x = gl::mul(__ldg(p.tab + (tg >> 1)), gl::MULT_GEN);
       if (tg & 1) x = gl::neg(x);
       den[r] = {gl::canon(gl::sub(x, p.at.c0)), neg_at1};
@@ -307,7 +311,47 @@ int32_t bj_deep_quotient_group(bj_ctx* ctx, const uint64_t* const* h_src_c0, con
   p.acc_c0 = (u64*)d_acc_c0;
   p.acc_c1 = (u64*)d_acc_c1;
   const u64 threads = (p.n_rows + DEEP_R - 1) / DEEP_R;
-  deep_group_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, ctx->stream>>>(p);
+  deep_group_kernel<false><<<(unsigned)((threads + 255) / 256), 256, 0, ctx->stream>>>(p);
+  BJ_LAUNCH_CHECK(ctx);
+  return BJ_OK;
+}
+
+int32_t bj_deep_quotient_range(bj_ctx* ctx, const uint64_t* const* h_src_c0, const uint64_t* const* h_src_c1, uint32_t n_src,
+                               const uint64_t* h_values_at, const uint64_t* h_challenges, const uint64_t h_at[2], uint32_t log_rows,
+                               uint64_t first_point, uint64_t n_points, uint64_t* d_acc_c0, uint64_t* d_acc_c1) {
+  bj::DeviceGuard device_guard(ctx);
+  if (!ctx || !h_src_c0 || !h_src_c1 || !h_values_at || !h_challenges || !h_at || !d_acc_c0 || !d_acc_c1 || n_src == 0 ||
+      log_rows < 1 || log_rows > 32 || n_points == 0 || first_point + n_points > (1ull << log_rows))
+    BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_deep_quotient_range: bad argument");
+  if (ctx->shard.log_stride) BJ_FAIL(ctx, BJ_ERR_UNSUPPORTED, "bj_deep_quotient_range: not on a sharded context");
+  BJ_TRY(ensure_twiddles(ctx, (int)log_rows));
+  DeepParams p;
+  std::vector<DeepColumn> cols;
+  cols.reserve(2 * (size_t)n_src);
+  gl::e2 k = {0, 0};
+  for (uint32_t i = 0; i < n_src; i++) {
+    const gl::e2 c = {gl::canon(h_challenges[2 * i]), gl::canon(h_challenges[2 * i + 1])};
+    const gl::e2 v = {gl::canon(h_values_at[2 * i]), gl::canon(h_values_at[2 * i + 1])};
+    if (!h_src_c0[i]) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_deep_quotient_range: NULL source column");
+    cols.push_back({(const u64*)h_src_c0[i], c.c0, c.c1});
+    if (h_src_c1[i]) cols.push_back({(const u64*)h_src_c1[i], gl::mul7(c.c1), c.c0});
+    const gl::e2 m = gl::e2_mul(c, v);
+    k = {gl::canon(gl::add(k.c0, m.c0)), gl::canon(gl::add(k.c1, m.c1))};
+  }
+  void* dcols;
+  BJ_TRY(param_upload(ctx, cols.data(), sizeof(DeepColumn) * cols.size(), &dcols));
+  p.cols = (const DeepColumn*)dcols;
+  p.n_cols = (u32)cols.size();
+  p.n_rows = n_points;
+  p.log_n = (int)log_rows;
+  p.tab = ctx->tw_fwd;
+  p.at = {gl::canon(h_at[0]), gl::canon(h_at[1])};
+  p.k_const = k;
+  p.acc_c0 = (u64*)d_acc_c0;
+  p.acc_c1 = (u64*)d_acc_c1;
+  p.first = first_point;
+  const u64 threads = (p.n_rows + DEEP_R - 1) / DEEP_R;
+  deep_group_kernel<true><<<(unsigned)((threads + 255) / 256), 256, 0, ctx->stream>>>(p);
   BJ_LAUNCH_CHECK(ctx);
   return BJ_OK;
 }

@@ -648,9 +648,13 @@ __global__ void __launch_bounds__(256) lde_unit_fold_kernel(const u64* __restric
   b[c * b_stride + k] = gl::canon(acc);
 }
 
-// bj_lde, and with next_row the LDE of f(w_n x) (every unit shift times w_n, same row order)
+// bj_lde, and with next_row the LDE of f(w_n x) (every unit shift times w_n, same row order).  cosets = {k0, k1} on an
+// unsharded context: only the cosets [k0, k1) (bj_lde_cosets), d_out [col][k1 - k0][row]
+struct CosetRange {
+  u64 k0, k1;
+};
 static int32_t lde_impl(bj_ctx* ctx, const uint64_t* d_in, uint64_t in_col_stride, uint64_t* d_out, uint32_t log_n, uint32_t log_lde,
-                        uint32_t n_cols, int32_t from_monomials, bool next_row) {
+                        uint32_t n_cols, int32_t from_monomials, bool next_row, const CosetRange* cosets = nullptr) {
   if (!ctx || !d_in || !d_out || log_n + log_lde > 32 || in_col_stride < (1ull << log_n))
     BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_lde: bad argument");
   if (n_cols == 0) return BJ_OK;
@@ -696,6 +700,7 @@ static int32_t lde_impl(bj_ctx* ctx, const uint64_t* d_in, uint64_t in_col_strid
     return BJ_OK;
   }
   const u64 L_loc = ctx->shard.local_units(L);  // cosets owned by this context (all of them without a shard)
+  const u64 k0 = cosets ? cosets->k0 : 0, k1 = cosets ? cosets->k1 : L_loc, n_out = k1 - k0;
   const int m = (int)log_n;
   // per chunk of columns: monomials (natural order) in scratch, then one forward transform per coset that
   // reads the monomials and writes straight into the coset's slot of d_out.
@@ -714,11 +719,11 @@ static int32_t lde_impl(bj_ctx* ctx, const uint64_t* d_in, uint64_t in_col_strid
       mono = mbuf;
       mono_stride = n;
     }
-    for (u64 k = 0; k < L_loc; k++) {
+    for (u64 k = k0; k < k1; k++) {
       u64 shift = ctx->shard.unit_shift(ctx->shard.global_unit(k), log_n, log_lde);  // the coset of local slot k
       if (next_row) shift = gl::mul(shift, w_row);
-      u64* out = (u64*)d_out + ((u64)c0 * L_loc + k) * n;
-      BJ_TRY(run_transform(ctx, mono, mono_stride, out, n * L_loc, m, cnt, shift, false, nullptr, 0));
+      u64* out = (u64*)d_out + ((u64)c0 * n_out + (k - k0)) * n;
+      BJ_TRY(run_transform(ctx, mono, mono_stride, out, n * n_out, m, cnt, shift, false, nullptr, 0));
     }
   }
   return BJ_OK;
@@ -738,6 +743,17 @@ int32_t bj_lde_next_row(bj_ctx* ctx, const uint64_t* d_in, uint64_t in_col_strid
                         uint32_t log_lde, uint32_t n_cols, int32_t from_monomials) {
   bj::DeviceGuard device_guard(ctx);
   return lde_impl(ctx, d_in, in_col_stride, d_out, log_n, log_lde, n_cols, from_monomials, true);
+}
+
+// LDE onto the cosets [coset_begin, coset_end) of the factor-2^log_lde domain only (unsharded contexts): the same coset
+// transforms as bj_lde, so every value is bit-identical to the matching slot of the full LDE.
+int32_t bj_lde_cosets(bj_ctx* ctx, const uint64_t* d_in, uint64_t in_col_stride, uint64_t* d_out, uint32_t log_n, uint32_t log_lde,
+                      uint32_t coset_begin, uint32_t coset_end, uint32_t n_cols, int32_t from_monomials) {
+  bj::DeviceGuard device_guard(ctx);
+  if (!ctx || coset_begin >= coset_end || log_lde > 32 || coset_end > (1ull << log_lde)) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_lde_cosets: bad argument");
+  if (ctx->shard.log_stride) BJ_FAIL(ctx, BJ_ERR_UNSUPPORTED, "bj_lde_cosets: not on a sharded context");
+  const CosetRange r{coset_begin, coset_end};
+  return lde_impl(ctx, d_in, in_col_stride, d_out, log_n, log_lde, n_cols, from_monomials, false, &r);
 }
 
 // Host-buffer entry points: the batch is cut into column chunks that flow through a 3-slot device ring, upload of chunk

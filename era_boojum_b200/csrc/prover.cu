@@ -12,8 +12,10 @@
 //   3  quotient, interpolation, chunks + oracle  :560-1495       6  queries                               :2161-2266
 #include <chrono>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <string>
+#include <unordered_map>
 #include <vector>
 #include "ctx.hpp"
 
@@ -39,7 +41,9 @@ struct DevMem {
     if (e != cudaSuccess) {
       cudaGetLastError();
       p = nullptr;
-      BJ_FAIL(c, BJ_ERR_OOM, "prover: device allocation failed");
+      uint64_t used = 0;
+      if (c->pool) cudaMemPoolGetAttribute(c->pool, cudaMemPoolAttrUsedMemCurrent, &used);
+      BJ_FAIL(c, BJ_ERR_OOM, "prover: device allocation of " + std::to_string(bytes) + " bytes failed (" + std::to_string(used) + " bytes of the pool in use)");
     }
     return BJ_OK;
   }
@@ -126,6 +130,57 @@ static int32_t lde_columns(bj_ctx* ctx, const uint64_t* d_in, uint64_t* d_out, u
   return finish(*groups.back());
 }
 
+// compact plan: the first `qn` elements (cosets [0, Q)) of every column, repacked with stride qn into `out`; cols is
+// repointed there.  The caller releases the full buffers.
+static int32_t keep_first_cosets(bj_ctx* ctx, std::vector<const uint64_t*>& cols, u64 qn, DevMem& out) {
+  BJ_TRY(out.alloc(ctx, cols.size() * qn));
+  for (size_t j = 0; j < cols.size(); j++) {
+    BJ_CUDA(ctx, cudaMemcpyAsync(out.p + j * qn, cols[j], sizeof(u64) * qn, cudaMemcpyDeviceToDevice, ctx->stream));
+    cols[j] = (const uint64_t*)out.p + j * qn;
+  }
+  return BJ_OK;
+}
+
+// compact plan: the witness and stage-2 LDEs are held as a few column groups, one allocation each, so that the repack to the
+// first Q cosets frees every group as soon as it is copied (the transient is one group's kept columns, not the oracle's)
+struct ColumnGroups {
+  std::vector<std::unique_ptr<DevMem>> full, kept;
+  std::vector<u32> cnt;
+};
+static constexpr u32 COMPACT_GROUPS = 4;
+static u32 compact_group_cols(u32 n_cols) { return (n_cols + COMPACT_GROUPS - 1) / COMPACT_GROUPS; }
+
+// LDE (one GPU) of n_cols natural columns of d_in onto all 2^log_d cosets, appended to g as groups; cols[j] = column j
+static int32_t lde_grouped(bj_ctx* ctx, ColumnGroups& g, const uint64_t* d_in, u32 n_cols, u32 log_n, u32 log_d, const uint64_t** cols) {
+  const u64 n = 1ull << log_n, nD = n << log_d;
+  const u32 per = compact_group_cols(n_cols);
+  for (u32 c0 = 0; c0 < n_cols; c0 += per) {
+    const u32 cnt = std::min(per, n_cols - c0);
+    g.full.emplace_back(new DevMem());
+    g.cnt.push_back(cnt);
+    BJ_TRY(g.full.back()->alloc(ctx, (size_t)cnt * nD));
+    BJ_TRY(bj_lde(ctx, d_in + (size_t)c0 * n, n, (uint64_t*)g.full.back()->p, log_n, log_d, cnt, 0));
+    for (u32 j = 0; j < cnt; j++) cols[c0 + j] = (const uint64_t*)g.full.back()->p + (size_t)j * nD;
+  }
+  return BJ_OK;
+}
+
+// keep_first_cosets group by group: cols (the groups' columns in order) is repointed to the kept copies
+static int32_t keep_first_cosets_grouped(bj_ctx* ctx, ColumnGroups& g, std::vector<const uint64_t*>& cols, u64 qn) {
+  size_t c0 = 0;
+  for (size_t k = 0; k < g.full.size(); k++) {
+    g.kept.emplace_back(new DevMem());
+    BJ_TRY(g.kept.back()->alloc(ctx, (size_t)g.cnt[k] * qn));
+    for (u32 j = 0; j < g.cnt[k]; j++) {
+      BJ_CUDA(ctx, cudaMemcpyAsync(g.kept.back()->p + (size_t)j * qn, cols[c0 + j], sizeof(u64) * qn, cudaMemcpyDeviceToDevice, ctx->stream));
+      cols[c0 + j] = (const uint64_t*)g.kept.back()->p + (size_t)j * qn;
+    }
+    g.full[k]->release();
+    c0 += g.cnt[k];
+  }
+  return BJ_OK;
+}
+
 int32_t copy_permutation_stage2_sharded(bj_ctx* ctx, const uint64_t* const* h_variable_cols, const uint64_t* const* h_sigma_cols, u32 n_cols,
                                         const uint64_t* h_non_residues, gl::e2 beta, gl::e2 gamma, u32 log_n, u32 chunk_size, u64* d_out);  // stage2.cu
 
@@ -189,6 +244,203 @@ struct QueryAnswer {
   std::vector<u64> path;  // 4 * depth
 };
 
+// ---- memory plan: the one owner of what bj_setup_create + bj_prove hold on the device at their peak ----
+// Two plans.  RESIDENT keeps every LDE column on all D = max(L, Q) cosets until the proof is done.  COMPACT (one GPU, Q < L)
+// keeps only the first Q cosets of the setup, witness and stage-2 columns once their trees are built: the quotient reads
+// cosets [0, Q) and the openings coset 0, so cosets [Q, L) are read by DEEP and the query answers only, and those two
+// recompute them from the natural-order columns, a chunk of columns and one coset at a time.  The quotient oracle stays
+// resident.  The plan replays the driver's stream-ordered pool allocations in order (pool_peak) and adds what the library
+// keeps outside the pool (library_reserve): twiddles, coset-power tables and the NTT scratch.
+struct ProofShape {
+  u32 V, C, T, W, n_s2, Q, L, log_n, log_l, log_d, log_q, world, split, cap, n_queries, sched_len;
+  u32 sched[32];
+  u64 n;
+  bool lk;
+  u32 nat_cols() const { return V + C + T + W + n_s2; }  // natural-order columns a compact proof recomputes from
+};
+
+static int32_t proof_shape(const bj_circuit& c, u32 world, ProofShape* s) {
+  auto lg = [](u32 x) { u32 l = 0; while ((1u << l) < x) l++; return l; };
+  s->V = c.num_variables;
+  s->C = c.num_constants;
+  s->lk = c.lookup_width != 0;
+  s->T = s->lk ? c.lookup_width + 1 : 0;
+  s->W = s->V + (s->lk ? 1 : 0);
+  s->Q = c.quotient_degree;
+  s->L = c.fri_lde_factor;
+  const u32 n_partial = (s->V + s->Q - 1) / s->Q - 1;
+  s->n_s2 = 2 + 2 * n_partial + (s->lk ? 2 * (c.lookup_num_repetitions + 1) : 0);
+  s->log_n = c.log_n;
+  s->log_l = lg(s->L);
+  s->log_q = lg(s->Q);
+  s->log_d = std::max(s->log_l, s->log_q);
+  s->world = world;
+  s->split = world > s->L ? lg(world) - s->log_l : 0;
+  s->cap = c.merkle_tree_cap_size;
+  s->n = 1ull << c.log_n;
+  u32 new_pow = 0, fd = 0;
+  return bj_compute_fri_schedule(c.security_level, c.merkle_tree_cap_size, c.pow_bits, s->log_l, c.log_n, &new_pow, &s->n_queries, s->sched,
+                                 &s->sched_len, &fd);
+}
+
+// bytes the context's pool counts as used for one allocation of n u64 (the requested size: DevMem asks for at least one)
+static inline u64 pool_bytes(u64 n_u64) { return sizeof(u64) * std::max<u64>(n_u64, 1); }
+
+struct Ledger {
+  u64 cur = 0, peak = 0;
+  void add(u64 n_u64) {
+    cur += pool_bytes(n_u64);
+    peak = std::max(peak, cur);
+  }
+  void sub(u64 n_u64) { cur -= pool_bytes(n_u64); }
+};
+
+// peak pool bytes of bj_setup_create followed by bj_prove; `chunk`: columns recomputed at a time (compact plan)
+static u64 pool_peak(const ProofShape& s, bool compact, u32 chunk) {
+  Ledger m;
+  const u64 n = s.n, w = s.world, nD = (n << s.log_d) / w, nL = (n << s.log_l) / w, nQ = n << s.log_q, Qn = n * s.Q;
+  const u64 leaves = (n << s.log_l) / w, capl = s.cap / w;
+  auto tree = [&]() {
+    m.add(4 * leaves);
+    m.add(4 * (leaves - capl));
+  };
+  auto lde_groups = [&](u32 cols) {  // lde_columns on a sharded context: at most two column groups of monomials at once
+    if (w == 1 || cols < 2) return;
+    const u64 group = std::max<u64>(w, ((cols + 3) / 4 + w - 1) / w * w), mono = w * ((group + w - 1) / w) * n;
+    const int alive = cols > group ? 2 : 1;
+    for (int i = 0; i < alive; i++) m.add(mono);
+    for (int i = 0; i < alive; i++) m.sub(mono);
+  };
+  const u64 S = s.V + s.C + s.T;
+  // bj_setup_create
+  m.add(S * nD);
+  lde_groups(s.V);
+  lde_groups(s.C);
+  lde_groups(s.T);
+  tree();
+  if (compact) {
+    m.add(S * Qn);
+    m.sub(S * nD);
+  }
+  // the compact plan's column groups (lde_grouped / keep_first_cosets_grouped): sizes of the groups of n_cols columns
+  auto groups = [](u32 n_cols) {
+    std::vector<u64> g;
+    for (u32 c0 = 0, per = compact_group_cols(n_cols); c0 < n_cols; c0 += per) g.push_back(std::min(per, n_cols - c0));
+    return g;
+  };
+  std::vector<u64> wg = groups(s.V), sg = groups(s.n_s2);
+  if (s.lk) wg.push_back(1);
+  // round 1
+  if (compact) {
+    for (u64 g : wg) m.add(g * nD);
+  } else {
+    m.add(s.V * nD);
+    lde_groups(s.V);
+    if (s.lk) m.add(nD);
+  }
+  tree();
+  if (compact)
+    for (u64 g : wg) {
+      m.add(g * Qn);
+      m.sub(g * nD);
+    }
+  // round 2
+  m.add(s.n_s2 * n);
+  if (compact) {
+    for (u64 g : sg) m.add(g * nD);
+  } else {
+    m.add(s.n_s2 * nD);
+    lde_groups(s.n_s2);
+  }
+  const u64 zn = s.split ? 2 * nD : 0;
+  if (zn) m.add(zn);
+  if (!compact) m.sub(s.n_s2 * n);  // the compact plan keeps the natural stage-2 columns for DEEP and the queries
+  tree();
+  if (compact)
+    for (u64 g : sg) {
+      m.add(g * Qn);
+      m.sub(g * nD);
+    }
+  // round 3
+  m.add(2 * nQ);
+  const u64 nQl = ((u64)s.Q << s.split) >= w ? nQ / w : n >> s.split;
+  if (w > 1) m.add(2 * std::max<u64>(nQl, 1));
+  if (zn) m.sub(zn);
+  if (w > 1) {
+    const u64 per = std::max<u64>(1, ((u64)s.Q << s.split) / w), nb = n >> s.split;
+    m.add(per * 2 * nb);
+    m.add(w * per * 2 * nb);
+    m.sub(w * per * 2 * nb);
+    m.sub(per * 2 * nb);
+    m.sub(2 * std::max<u64>(nQl, 1));
+  }
+  m.add(2 * nQ);  // chunks
+  m.sub(2 * nQ);  // qq
+  m.add(2 * (u64)s.Q * nL);
+  m.sub(2 * nQ);  // chunks
+  tree();
+  // round 5
+  m.add(2 * nL);
+  if (compact) {  // DEEP on the dropped cosets: monomials + one coset of a chunk of columns
+    m.add((u64)chunk * n);
+    m.add((u64)chunk * n);
+    m.sub((u64)chunk * n);
+    m.sub((u64)chunk * n);
+  }
+  u64 log_m = s.log_n + s.log_l;
+  u32 kmax = 0;
+  for (u32 i = 0; i < s.sched_len; i++) {
+    const u32 k = s.sched[i];
+    kmax = std::max(kmax, k);
+    const u64 lv_leaves = (1ull << (log_m - k)) / w;
+    m.add(4 * lv_leaves);
+    m.add(4 * (lv_leaves - capl));
+    m.add((1ull << (log_m - k)) / w);
+    m.add((1ull << (log_m - k)) / w);
+    log_m -= k;
+  }
+  const u64 fft = 1ull << log_m;
+  m.add(fft);
+  m.add(fft);
+  if (w > 1) {
+    m.add(2 * fft / w);
+    m.add(2 * fft);
+    m.sub(2 * fft);
+    m.sub(2 * fft / w);
+  }
+  m.sub(fft);
+  m.sub(fft);
+  // queries: one gather buffer at a time (leaf rows, Merkle paths, FRI leaves); the compact plan then recomputes the rows
+  // of the dropped cosets chunk by chunk
+  u32 depth = 0;
+  while ((leaves >> depth) > capl) depth++;
+  const u64 row_max = std::max<u64>({S, s.W, s.n_s2, 2 * (u64)s.Q, 4 * (u64)depth, 2ull << kmax});
+  m.add((u64)s.n_queries * row_max);
+  m.sub((u64)s.n_queries * row_max);
+  if (compact) {
+    m.add((u64)chunk * n);
+    m.add((u64)chunk * n);
+    m.add((u64)s.n_queries * chunk);
+  }
+  return m.peak;
+}
+
+// device bytes the library holds outside the pool during a proof (upper bounds): forward + inverse twiddles of the
+// factor-D domain, the coset-power tables (capped by their 3 GiB budget in ntt.cu), the NTT / LDE / opening scratch, and a
+// fixed 16 MiB for the parameter arena (8 MiB) and the long gate programs gates.cu uploads outside the context's pool
+static u64 library_reserve(const ProofShape& s) {
+  const u64 n = s.n, D = 1ull << s.log_d;
+  u64 r = sizeof(u64) * n * D;
+  r += std::min<u64>(3ull << 30, sizeof(u64) * n * (D + s.Q + 2)) + 64 * 16 * (1ull << ((s.log_n + s.log_d + 2) / 2));
+  r += sizeof(u64) * std::max<u64>(1ull << 27, 4 * n);
+  r += 16ull << 20;
+  return r;
+}
+
+static bool compact_applies(const ProofShape& s) { return s.world == 1 && s.Q < s.L; }
+
+static u64 plan_bytes(const ProofShape& s, bool compact, u32 chunk = 2) { return pool_peak(s, compact, chunk) + library_reserve(s); }
+
 }  // namespace bj
 
 struct bj_setup {
@@ -201,7 +453,13 @@ struct bj_setup {
   uint32_t n_tables = 0;
   bj::DevMem lde;  // [V + C + T][D][n], D = max(L, quotient degree): the tree commits to the first L cosets of every column
   bj::Oracle tree;
-  uint64_t col_len = 0;  // elements of one LDE column held by this context: n * (D / world)
+  uint64_t col_len = 0;  // elements of one LDE column held by this context: n * (D / world), or n * Q on the compact plan
+  bool compact = false;  // memory plan chosen by bj_setup_create, followed by bj_prove
+  uint64_t limit = 0;    // the device-memory limit the plan was chosen under
+  uint64_t plan[2] = {0, 0};  // resident, compact (0: no compact plan)
+  uint32_t chunk = 2;         // compact plan: natural-order columns recomputed at a time
+  uint64_t pool_bytes = 0, outside_pool_bytes = 0;  // the chosen plan (with its chunk): pool peak, library reserve
+  uint64_t chosen_bytes() const { return pool_bytes + outside_pool_bytes; }
   const uint64_t* col(uint32_t j) const { return (const uint64_t*)lde.p + (size_t)j * col_len; }
   uint32_t log_l() const {
     uint32_t l = 0;
@@ -236,6 +494,30 @@ struct bj_proof {
 using namespace bj;
 
 static bool is_pow2(uint32_t x) { return x && !(x & (x - 1)); }
+
+// the limit a plan must fit under: the one set on the context, or what the device has free plus what the context's pool
+// holds without using it
+static int32_t memory_limit(bj_ctx* ctx, uint64_t* out) {
+  if (ctx->memory_limit) {
+    *out = ctx->memory_limit;
+    return BJ_OK;
+  }
+  size_t free_b = 0, total_b = 0;
+  BJ_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
+  uint64_t reserved = 0, used = 0;
+  if (ctx->pool) {
+    BJ_CUDA(ctx, cudaMemPoolGetAttribute(ctx->pool, cudaMemPoolAttrReservedMemCurrent, &reserved));
+    BJ_CUDA(ctx, cudaMemPoolGetAttribute(ctx->pool, cudaMemPoolAttrUsedMemCurrent, &used));
+  }
+  *out = free_b + (reserved > used ? reserved - used : 0);
+  return BJ_OK;
+}
+
+static std::string plan_message(const char* who, const uint64_t plan[2], uint64_t limit) {
+  std::string m = std::string(who) + ": the proof needs " + std::to_string(plan[0]) + " bytes of device memory resident";
+  m += plan[1] ? " and " + std::to_string(plan[1]) + " bytes on the compact plan" : std::string(" (no compact plan: sharded context or quotient degree >= LDE factor)");
+  return m + ", above the limit of " + std::to_string(limit) + " bytes";
+}
 
 extern "C" {
 
@@ -280,6 +562,30 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
     }
   }
   std::unique_ptr<bj_setup> s(new bj_setup());
+  {
+    // the memory plan: resident if it fits under the limit, compact otherwise; refused before anything is launched
+    ProofShape sh;
+    BJ_TRY(proof_shape(*circuit, comm_world(ctx), &sh));
+    s->plan[0] = plan_bytes(sh, false);
+    s->plan[1] = compact_applies(sh) ? plan_bytes(sh, true) : 0;
+    BJ_TRY(memory_limit(ctx, &s->limit));
+    if (s->plan[0] > s->limit) {
+      if (!s->plan[1] || s->plan[1] > s->limit) BJ_FAIL(ctx, BJ_ERR_OOM, plan_message("bj_setup_create", s->plan, s->limit));
+      s->compact = true;
+      // wider recompute chunks only save kernel launches: the chunk grows into at most half of the headroom the limit leaves
+      // over the plan (the rest is slack for the pool's fragmentation) and stops at 16 columns
+      const uint64_t budget = s->plan[1] + (s->limit - s->plan[1]) / 2;
+      uint32_t lo = 2, hi = std::max<uint32_t>(2, std::min<uint32_t>(16, sh.nat_cols()));
+      while (lo < hi) {
+        const uint32_t mid = lo + (hi - lo + 1) / 2;
+        if (plan_bytes(sh, true, mid) <= budget) lo = mid;
+        else hi = mid - 1;
+      }
+      s->chunk = lo;
+    }
+    s->pool_bytes = pool_peak(sh, s->compact, s->chunk);
+    s->outside_pool_bytes = library_reserve(sh);
+  }
   s->ctx = ctx;
   s->c = *circuit;
   // deep copy of the gate programs (the caller's arrays need not outlive this call)
@@ -321,6 +627,12 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
   if (T) BJ_TRY(lde_columns(ctx, d_lookup_tables, (uint64_t*)s->lde.p + (size_t)(V + C) * s->col_len, log_n, log_d, T));
   for (uint32_t j = 0; j < V + C + T; j++) s->tree.cols.push_back(s->col(j));
   BJ_TRY(oracle_build(ctx, s->tree, n << log_l, circuit->merkle_tree_cap_size, circuit->tree_hasher, circuit->fri_lde_factor));
+  if (s->compact) {
+    DevMem kept;
+    BJ_TRY(keep_first_cosets(ctx, s->tree.cols, n * circuit->quotient_degree, kept));
+    std::swap(s->lde.p, kept.p);
+    s->col_len = n * circuit->quotient_degree;
+  }
   *out = s.release();
   return BJ_OK;
 }
@@ -360,7 +672,17 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   const u64 nQl = ctx->shard.local_points(Q, (int)log_n);                 // LOCAL quotient points
   const uint32_t split = ctx->shard.log_split;                            // 2^split row blocks per coset (split domain shard)
   const u64 nb = n >> split;                                             // rows of one unit
-  if (setup->col_len != nD) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: the setup was built with a different shard");
+  const bool compact = setup->compact;
+  const u64 Qn = n * Q;  // compact plan: elements of a setup / witness / stage-2 column kept on the device (cosets [0, Q))
+  if (setup->col_len != (compact ? Qn : nD)) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: the setup was built with a different shard");
+  const uint32_t chunk = setup->chunk;  // compact plan: natural-order columns recomputed at a time
+  {
+    const uint64_t limit = ctx->memory_limit ? ctx->memory_limit : setup->limit;
+    if (setup->chosen_bytes() > limit) BJ_FAIL(ctx, BJ_ERR_OOM, plan_message("bj_prove", setup->plan, limit));
+  }
+  // Every DevMem below (and the FRI / query buffers of fri_driver.cu) is replayed by pool_peak in the same order: a new
+  // allocation here must be added there, or the plan no longer bounds the pool (tests/test_gpu_memory_budget.py pins the
+  // pool's high-water mark to the plan).
   const uint32_t T = setup->n_tables, wdt = c.lookup_width, nsub = c.lookup_num_repetitions, voff = c.lookup_variables_offset;
   auto t_prev = std::chrono::steady_clock::now();
   auto mark = [&](int stage) -> int32_t {
@@ -397,20 +719,33 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
 
   // ---- round 1: witness commitment ----
   DevMem w_lde, m_lde;
-  BJ_TRY(w_lde.alloc(ctx, (size_t)V * nD));
-  BJ_TRY(lde_columns(ctx, d_variables, (uint64_t*)w_lde.p, log_n, log_d, V));
+  ColumnGroups w_groups;  // compact plan
   std::vector<const uint64_t*> w_cols(V);
-  for (uint32_t j = 0; j < V; j++) w_cols[j] = (const uint64_t*)w_lde.p + (size_t)j * nD;
+  const uint64_t* m_col = nullptr;
+  if (compact) {
+    BJ_TRY(lde_grouped(ctx, w_groups, d_variables, V, log_n, log_d, w_cols.data()));
+    if (lk) BJ_TRY(lde_grouped(ctx, w_groups, d_multiplicities, 1, log_n, log_d, &m_col));
+  } else {
+    BJ_TRY(w_lde.alloc(ctx, (size_t)V * nD));
+    BJ_TRY(lde_columns(ctx, d_variables, (uint64_t*)w_lde.p, log_n, log_d, V));
+    for (uint32_t j = 0; j < V; j++) w_cols[j] = (const uint64_t*)w_lde.p + (size_t)j * nD;
+    if (lk) {
+      BJ_TRY(m_lde.alloc(ctx, nD));
+      BJ_TRY(bj_lde(ctx, d_multiplicities, n, (uint64_t*)m_lde.p, log_n, log_d, 1, 0));
+      m_col = (const uint64_t*)m_lde.p;
+    }
+  }
   Oracle w_or;
   w_or.cols = w_cols;
-  if (lk) {
-    BJ_TRY(m_lde.alloc(ctx, nD));
-    BJ_TRY(bj_lde(ctx, d_multiplicities, n, (uint64_t*)m_lde.p, log_n, log_d, 1, 0));
-    w_or.cols.push_back((const uint64_t*)m_lde.p);  // variables | witness (none) | multiplicities
-  }
+  if (lk) w_or.cols.push_back(m_col);  // variables | witness (none) | multiplicities
   BJ_TRY(oracle_build(ctx, w_or, n << log_l, cap, c.tree_hasher, L));
   pf->witness_cap = w_or.cap;
   bj_transcript_witness_merkle_tree_cap(tr, (const uint64_t*)w_or.cap.data(), cap);
+  if (compact) {
+    BJ_TRY(keep_first_cosets_grouped(ctx, w_groups, w_or.cols, Qn));
+    for (uint32_t j = 0; j < V; j++) w_cols[j] = w_or.cols[j];
+    if (lk) m_col = w_or.cols[V];
+  }
   BJ_TRY(mark(0));
 
   // ---- round 2: copy-permutation grand product, partial products, lookup polynomials ----
@@ -447,8 +782,15 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
                                          d_multiplicities, lb, lg, log_n, (uint64_t*)st2.p + (size_t)(2 + 2 * n_partial) * n));
     }
   }
-  BJ_TRY(s2_lde.alloc(ctx, (size_t)n_s2 * nD));
-  BJ_TRY(lde_columns(ctx, (const uint64_t*)st2.p, (uint64_t*)s2_lde.p, log_n, log_d, n_s2));
+  ColumnGroups s2_groups;  // compact plan
+  std::vector<const uint64_t*> s2_cols(n_s2);
+  if (compact) {
+    BJ_TRY(lde_grouped(ctx, s2_groups, (const uint64_t*)st2.p, n_s2, log_n, log_d, s2_cols.data()));
+  } else {
+    BJ_TRY(s2_lde.alloc(ctx, (size_t)n_s2 * nD));
+    BJ_TRY(lde_columns(ctx, (const uint64_t*)st2.p, (uint64_t*)s2_lde.p, log_n, log_d, n_s2));
+    for (uint32_t j = 0; j < n_s2; j++) s2_cols[j] = (const uint64_t*)s2_lde.p + (size_t)j * nD;
+  }
   // a row block of a split shard does not hold z(omega x) (another block of the coset does).  On a unit with shift sigma,
   // z(omega x) is the LDE of z on the shift sigma * omega in the same row order: two more columns (c0, c1 of z)
   DevMem z_next;
@@ -456,14 +798,16 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     BJ_TRY(z_next.alloc(ctx, 2 * nD));
     BJ_TRY(bj_lde_next_row(ctx, (const uint64_t*)st2.p, n, (uint64_t*)z_next.p, log_n, log_d, 2, 0));
   }
-  st2.release();
-  std::vector<const uint64_t*> s2_cols(n_s2);
-  for (uint32_t j = 0; j < n_s2; j++) s2_cols[j] = (const uint64_t*)s2_lde.p + (size_t)j * nD;
+  if (!compact) st2.release();  // the compact plan recomputes cosets [Q, L) of stage 2 from it
   Oracle s2_or;
   s2_or.cols = s2_cols;
   BJ_TRY(oracle_build(ctx, s2_or, n << log_l, cap, c.tree_hasher, L));
   pf->stage2_cap = s2_or.cap;
   bj_transcript_witness_merkle_tree_cap(tr, (const uint64_t*)s2_or.cap.data(), cap);
+  if (compact) {
+    BJ_TRY(keep_first_cosets_grouped(ctx, s2_groups, s2_or.cols, Qn));
+    s2_cols = s2_or.cols;
+  }
   const uint32_t a_off = 2 + 2 * n_partial;
   BJ_TRY(mark(1));
 
@@ -507,7 +851,7 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     for (uint32_t i = 0; i < 2 * nsub; i++) al[i] = s2_cols[a_off + i];
     const uint64_t lb[2] = {lookup_beta.c0, lookup_beta.c1}, lg[2] = {lookup_gamma.c0, lookup_gamma.c1};
     BJ_TRY(bj_quotient_lookup_specialized(ctx, ll.data(), nsub, wdt, const_cols[c.lookup_table_id_column], table_cols.data(), T,
-                                          (const uint64_t*)m_lde.p, al.data(), s2_cols[a_off + 2 * nsub], s2_cols[a_off + 2 * nsub + 1], lb, lg,
+                                          m_col, al.data(), s2_cols[a_off + 2 * nsub], s2_cols[a_off + 2 * nsub + 1], lb, lg,
                                           powers.data(), nQl, q0, q1));
   }
   if (n_gate_terms)
@@ -602,7 +946,7 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   for (uint32_t i = 0; i < 1 + n_partial; i++) sources.push_back({s2_cols[2 * i], s2_cols[2 * i + 1]});
   std::vector<Src> zero_sources;
   if (lk) {
-    sources.push_back({(const uint64_t*)m_lde.p, nullptr});
+    sources.push_back({m_col, nullptr});
     for (uint32_t i = 0; i < nsub + 1; i++) {
       sources.push_back({s2_cols[a_off + 2 * i], s2_cols[a_off + 2 * i + 1]});
       zero_sources.push_back({s2_cols[a_off + 2 * i], s2_cols[a_off + 2 * i + 1]});
@@ -697,8 +1041,79 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   DevMem deep;
   BJ_TRY(deep.alloc(ctx, 2 * nL));
   BJ_CUDA(ctx, cudaMemsetAsync(deep.p, 0, sizeof(u64) * 2 * nL, ctx->stream));
+  // compact plan: the natural-order columns behind the setup, witness and stage-2 oracles, in the order of the oracles'
+  // columns (so a row of them is the three oracles' leaves side by side), and the kept LDE column of each
+  std::vector<const uint64_t*> nat;
+  std::unordered_map<const uint64_t*, uint32_t> nat_of;  // kept LDE column -> its index in nat
+  std::vector<char> pair_start;                          // nat[i], nat[i + 1] are the c0, c1 of one Fp2 polynomial
+  const uint32_t S = V + C + T;
+  if (compact) {
+    for (uint32_t j = 0; j < V; j++) nat.push_back(setup->sigmas + (size_t)j * n);
+    for (uint32_t j = 0; j < C; j++) nat.push_back(setup->constants + (size_t)j * n);
+    for (uint32_t j = 0; j < T; j++) nat.push_back(setup->tables + (size_t)j * n);
+    for (uint32_t j = 0; j < V; j++) nat.push_back(d_variables + (size_t)j * n);
+    if (lk) nat.push_back(d_multiplicities);
+    for (uint32_t j = 0; j < n_s2; j++) nat.push_back((const uint64_t*)st2.p + (size_t)j * n);
+    std::vector<const uint64_t*> kept(setup->tree.cols);
+    kept.insert(kept.end(), w_or.cols.begin(), w_or.cols.end());
+    kept.insert(kept.end(), s2_or.cols.begin(), s2_or.cols.end());
+    for (uint32_t i = 0; i < kept.size(); i++) nat_of[kept[i]] = i;
+    pair_start.assign(nat.size(), 0);
+    for (uint32_t j = 0; j < n_s2; j += 2) pair_start[S + w_or.cols.size() + j] = 1;
+  }
+  // chunks of `chunk` natural columns (an Fp2 pair never split): monomials by one iNTT, then body(c0, cnt, monomials, scratch
+  // for one coset of the chunk)
+  auto for_chunks = [&](const std::function<int32_t(uint32_t, uint32_t, const uint64_t*, uint64_t*)>& body) -> int32_t {
+    DevMem mono, ev;
+    BJ_TRY(mono.alloc(ctx, (size_t)chunk * n));
+    BJ_TRY(ev.alloc(ctx, (size_t)chunk * n));
+    for (uint32_t c0 = 0; c0 < nat.size();) {
+      uint32_t cnt = std::min<uint32_t>(chunk, (uint32_t)nat.size() - c0);
+      if (c0 + cnt < nat.size() && pair_start[c0 + cnt - 1]) cnt--;
+      for (uint32_t i = 0; i < cnt; i++)
+        BJ_CUDA(ctx, cudaMemcpyAsync(mono.p + (size_t)i * n, nat[c0 + i], sizeof(u64) * n, cudaMemcpyDeviceToDevice, ctx->stream));
+      BJ_TRY(bj_intt_natural_to_natural(ctx, (uint64_t*)mono.p, log_n, cnt, n, 1));
+      BJ_TRY(body(c0, cnt, (const uint64_t*)mono.p, (uint64_t*)ev.p));
+      c0 += cnt;
+    }
+    return BJ_OK;
+  };
+  struct DeepGroup {
+    const std::vector<Src>* srcs;
+    const std::vector<gl::e2>* vals;
+    gl::e2 at;
+    const uint64_t* chs;
+  };
+  std::vector<DeepGroup> deep_groups;
+  // sources i of a group with keep(i) on the points [first, first + count), column pointers moved by col_off(i)
+  auto deep_range = [&](const DeepGroup& g, const std::function<bool(size_t)>& keep, const std::function<const uint64_t*(const uint64_t*)>& at_col,
+                        u64 first, u64 count) -> int32_t {
+    std::vector<const uint64_t*> p0, p1;
+    std::vector<uint64_t> v, ch;
+    for (size_t i = 0; i < g.srcs->size(); i++) {
+      if (!keep(i)) continue;
+      const Src& sr = (*g.srcs)[i];
+      p0.push_back(at_col(sr.c0));
+      p1.push_back(sr.c1 ? at_col(sr.c1) : nullptr);
+      v.push_back((*g.vals)[i].c0);
+      v.push_back((*g.vals)[i].c1);
+      ch.push_back(g.chs[2 * i]);
+      ch.push_back(g.chs[2 * i + 1]);
+    }
+    if (p0.empty()) return BJ_OK;
+    const uint64_t a[2] = {g.at.c0, g.at.c1};
+    return bj_deep_quotient_range(ctx, p0.data(), p1.data(), (uint32_t)p0.size(), v.data(), ch.data(), a, log_n + log_l, first, count,
+                                  (uint64_t*)deep.p + first, (uint64_t*)deep.p + nL + first);
+  };
   auto deep_group = [&](const std::vector<Src>& srcs, const std::vector<gl::e2>& vals, gl::e2 at, const uint64_t* chs) -> int32_t {
     if (srcs.empty()) return BJ_OK;
+    if (compact) {
+      // cosets [0, Q) from the kept columns; the quotient oracle's columns hold all L cosets; the rest is recomputed below
+      const DeepGroup g{&srcs, &vals, at, chs};
+      deep_groups.push_back(g);
+      BJ_TRY(deep_range(g, [](size_t) { return true; }, [](const uint64_t* p) { return p; }, 0, Qn));
+      return deep_range(g, [&](size_t i) { return !nat_of.count(srcs[i].c0); }, [&](const uint64_t* p) { return p + Qn; }, Qn, nL - Qn);
+    }
     std::vector<const uint64_t*> p0(srcs.size()), p1(srcs.size());
     std::vector<uint64_t> v(2 * srcs.size());
     for (size_t i = 0; i < srcs.size(); i++) {
@@ -721,6 +1136,20 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
       off += g.srcs.size();
     }
   }
+  if (compact)  // cosets [Q, L): every chunk of natural columns evaluated on one coset at a time, its DEEP terms added
+    BJ_TRY(for_chunks([&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* ev) -> int32_t {
+      auto in_chunk = [&](const uint64_t* p) {
+        const auto it = nat_of.find(p);
+        return it != nat_of.end() && it->second >= c0 && it->second < c0 + cnt;
+      };
+      auto on_coset = [&](const uint64_t* p) -> const uint64_t* { return ev + (size_t)(nat_of.at(p) - c0) * n; };
+      for (uint32_t j = Q; j < L; j++) {
+        BJ_TRY(bj_lde_cosets(ctx, mono, n, ev, log_n, log_l, j, j + 1, cnt, 1));
+        for (const DeepGroup& g : deep_groups)
+          BJ_TRY(deep_range(g, [&](size_t i) { return in_chunk((*g.srcs)[i].c0); }, on_coset, (u64)j * n, n));
+      }
+      return BJ_OK;
+    }));
   uint32_t new_pow = 0, num_queries = 0, sched[32], sched_len = 0, final_degree = 0;
   BJ_TRY(bj_compute_fri_schedule(c.security_level, cap, c.pow_bits, log_l, log_n, &new_pow, &num_queries, sched, &sched_len, &final_degree));
   bj_fri_oracles* fri = nullptr;
@@ -780,12 +1209,49 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     while ((o->n_leaves >> depth) > o->cap_size) depth++;
     Part rows{std::vector<uint64_t>((size_t)num_queries * row_len), row_len};
     Part path{std::vector<uint64_t>((size_t)num_queries * depth * 4), (size_t)depth * 4};
-    BJ_TRY(bj_query_leaf_elements(ctx, o->cols.data(), (uint32_t)row_len, 1, o->n_leaves, loc_idx.data(), num_queries, rows.data.data()));
+    if (compact && o != &qt_or) {  // kept columns hold cosets [0, Q); the rows of the other cosets are recomputed below
+      std::vector<uint64_t> kept_idx(loc_idx);
+      for (auto& i : kept_idx)
+        if (i >= Qn) i = 0;
+      BJ_TRY(bj_query_leaf_elements(ctx, o->cols.data(), (uint32_t)row_len, 1, Qn, kept_idx.data(), num_queries, rows.data.data()));
+    } else {
+      BJ_TRY(bj_query_leaf_elements(ctx, o->cols.data(), (uint32_t)row_len, 1, o->n_leaves, loc_idx.data(), num_queries, rows.data.data()));
+    }
     if (depth)
       BJ_TRY(bj_merkle_paths(ctx, (const uint64_t*)o->leaf_hashes.p, (const uint64_t*)o->nodes.p, o->n_leaves, o->cap_size, loc_idx.data(),
                              num_queries, path.data.data()));
     parts.push_back(std::move(rows));
     parts.push_back(std::move(path));
+  }
+  if (compact) {
+    // queries whose leaf lies in a dropped coset j: one recompute of each such coset per chunk, the queried rows gathered
+    // from it.  Natural column i belongs to the setup (rows in parts[6]), witness (parts[0]) or stage-2 (parts[2]) oracle.
+    std::vector<std::vector<uint32_t>> by_coset(L);
+    for (uint32_t q = 0; q < num_queries; q++)
+      if (idxs[q] >= Qn) by_coset[idxs[q] / n].push_back(q);
+    bool any = false;
+    for (uint32_t j = Q; j < L; j++) any = any || !by_coset[j].empty();
+    const uint32_t Wc = (uint32_t)w_or.cols.size();
+    if (any)
+      BJ_TRY(for_chunks([&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* ev) -> int32_t {
+        std::vector<const uint64_t*> cols(cnt);
+        for (uint32_t i = 0; i < cnt; i++) cols[i] = ev + (size_t)i * n;
+        for (uint32_t j = Q; j < L; j++) {
+          const auto& qs = by_coset[j];
+          if (qs.empty()) continue;
+          BJ_TRY(bj_lde_cosets(ctx, mono, n, ev, log_n, log_l, j, j + 1, cnt, 1));
+          std::vector<uint64_t> rows_in(qs.size()), got(qs.size() * (size_t)cnt);
+          for (size_t k = 0; k < qs.size(); k++) rows_in[k] = idxs[qs[k]] - (u64)j * n;
+          BJ_TRY(bj_query_leaf_elements(ctx, cols.data(), cnt, 1, n, rows_in.data(), (uint32_t)qs.size(), got.data()));
+          for (uint32_t i = 0; i < cnt; i++) {
+            const uint32_t col = c0 + i;
+            Part& pt = col < S ? parts[6] : col < S + Wc ? parts[0] : parts[2];
+            const uint32_t within = col < S ? col : col < S + Wc ? col - S : col - S - Wc;
+            for (size_t k = 0; k < qs.size(); k++) pt.data[(size_t)qs[k] * pt.rec_len + within] = got[k * cnt + i];
+          }
+        }
+        return BJ_OK;
+      }));
   }
   {
     uint32_t log_len = log_n;  // coset length of the level's codeword
@@ -895,6 +1361,29 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   }
   s += "],\"pow_challenge\":" + std::to_string(pf->pow_challenge) + ",\"_marker\":null}";
   *out = pf.release();
+  return BJ_OK;
+}
+
+int32_t bj_proof_memory_plan(const bj_circuit* circuit, uint32_t world, uint64_t out[2]) {
+  if (!circuit || !out || world == 0 || (world & (world - 1)) || circuit->log_n == 0 || circuit->log_n > 28 || !is_pow2(circuit->fri_lde_factor) ||
+      circuit->fri_lde_factor < 2 || !is_pow2(circuit->quotient_degree) || !is_pow2(circuit->merkle_tree_cap_size) ||
+      circuit->merkle_tree_cap_size < world || circuit->num_variables == 0)
+    return BJ_ERR_INVALID_ARG;
+  ProofShape sh;
+  BJ_TRY(proof_shape(*circuit, world, &sh));
+  if (sh.sched_len == 0) return BJ_ERR_INVALID_ARG;
+  out[0] = plan_bytes(sh, false);
+  out[1] = compact_applies(sh) ? plan_bytes(sh, true) : 0;
+  return BJ_OK;
+}
+
+int32_t bj_setup_is_compact(const bj_setup* s) { return s ? (s->compact ? 1 : 0) : BJ_ERR_INVALID_ARG; }
+
+int32_t bj_setup_memory_plan(const bj_setup* s, uint64_t out[3]) {
+  if (!s || !out) return BJ_ERR_INVALID_ARG;
+  out[0] = s->pool_bytes;
+  out[1] = s->outside_pool_bytes;
+  out[2] = s->compact ? s->chunk : 0;
   return BJ_OK;
 }
 

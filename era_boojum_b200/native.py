@@ -49,6 +49,8 @@ SIGNATURES = {
     "bj_ctx_synchronize": (_i32, [_vp]),
     "bj_last_error": (ctypes.c_char_p, [_vp]),
     "bj_launch_count": (_u64, [_vp]),
+    "bj_ctx_set_memory_limit": (_i32, [_vp, _u64]),
+    "bj_ctx_memory_high_water": (_i32, [_vp, _vp, _i32]),
     "bj_alloc": (_i32, [_vp, _sz, _pp]),
     "bj_free": (_i32, [_vp, _vp]),
     "bj_upload": (_i32, [_vp, _vp, _vp, _sz]),
@@ -61,6 +63,7 @@ SIGNATURES = {
     "bj_bitreverse": (_i32, [_vp, _vp, _u32, _u32, _u64]),
     "bj_lde": (_i32, [_vp, _vp, _u64, _vp, _u32, _u32, _u32, _i32]),
     "bj_lde_next_row": (_i32, [_vp, _vp, _u64, _vp, _u32, _u32, _u32, _i32]),
+    "bj_lde_cosets": (_i32, [_vp, _vp, _u64, _vp, _u32, _u32, _u32, _u32, _u32, _i32]),
     "bj_merkle_build_poseidon2": (_i32, [_vp, _vp, _u32, _u64, _u32, _u32, _vp, _vp]),
     "bj_merkle_build_blake2s": (_i32, [_vp, _vp, _u32, _u64, _u32, _u32, _vp, _vp]),
     "bj_merkle_build_keccak256": (_i32, [_vp, _vp, _u32, _u64, _u32, _u32, _vp, _vp]),
@@ -70,6 +73,7 @@ SIGNATURES = {
     "bj_batch_inverse": (_i32, [_vp, _vp, _u64]),
     "bj_batch_inverse_ext": (_i32, [_vp, _vp, _vp, _u64]),
     "bj_deep_quotient_group": (_i32, [_vp, _vp, _vp, _u32, _vp, _vp, _vp, _u32, _vp, _vp]),
+    "bj_deep_quotient_range": (_i32, [_vp, _vp, _vp, _u32, _vp, _vp, _vp, _u32, _u64, _u64, _vp, _vp]),
     "bj_non_residues_for_copy_permutation": (_i32, [_u64, _u32, _vp]),
     "bj_copy_permutation_stage2": (_i32, [_vp, _vp, _vp, _u32, _vp, _vp, _vp, _u32, _u32, _vp, _vp, _vp]),
     "bj_quotient_copy_permutation": (_i32, [_vp, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _u32, _u32, _vp, _vp]),
@@ -121,6 +125,9 @@ SIGNATURES = {
     "bj_comm_broadcast_host": (_i32, [_vp, _vp, _u64, _u32]),
     "bj_setup_create": (_i32, [_vp, _vp, _vp, _vp, _vp, _pp]),
     "bj_setup_free": (None, [_vp]),
+    "bj_proof_memory_plan": (_i32, [_vp, _u32, _vp]),
+    "bj_setup_is_compact": (_i32, [_vp]),
+    "bj_setup_memory_plan": (_i32, [_vp, _vp]),
     "bj_setup_get_cap": (_i32, [_vp, _vp]),
     "bj_prove": (_i32, [_vp, _vp, _vp, _vp, _pp]),
     "bj_proof_free": (None, [_vp]),

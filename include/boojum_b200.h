@@ -77,6 +77,15 @@ BJ_API int32_t bj_ctx_set_domain_shard(bj_ctx* ctx, uint32_t rank, uint32_t worl
 BJ_API const char* bj_last_error(const bj_ctx* ctx);
 /* number of kernels this library launched through ctx so far (for launch accounting) */
 BJ_API uint64_t bj_launch_count(const bj_ctx* ctx);
+/* Device-memory limit of the prover driver on this context (bytes; 0, the default: what the device has free when
+ * bj_setup_create runs, plus what the context's pool holds without using it).  bj_setup_create compares the two memory plans
+ * of bj_proof_memory_plan with it: RESIDENT if that fits, else COMPACT (one GPU, quotient degree < LDE factor), else
+ * BJ_ERR_OOM with both byte counts in the message and no kernel launched.  bj_prove follows the setup's plan and refuses the
+ * same way if the limit was lowered below it since. */
+BJ_API int32_t bj_ctx_set_memory_limit(bj_ctx* ctx, uint64_t bytes);
+/* highest device memory the context's pool has had in use (cudaMemPoolAttrUsedMemHigh); reset != 0 restarts the mark.
+ * Synchronises.  Memory the library keeps outside the pool (twiddles, coset-power tables, scratch) is not included. */
+BJ_API int32_t bj_ctx_memory_high_water(bj_ctx* ctx, uint64_t* bytes, int32_t reset);
 
 /* ---- multi-GPU: communicator of the sharded prover (one process - or one thread - per GPU) ----
  * Creating a communicator on a context declares its domain shard (bj_ctx_set_domain_shard(ctx, rank, world, log_lde)) and makes
@@ -150,6 +159,10 @@ BJ_API int32_t bj_lde(bj_ctx* ctx, const uint64_t* d_in, uint64_t in_col_stride,
  * shard reads z(omega x) of the copy-permutation quotient from here (the row itself lives in another block). */
 BJ_API int32_t bj_lde_next_row(bj_ctx* ctx, const uint64_t* d_in, uint64_t in_col_stride, uint64_t* d_out, uint32_t log_n,
                                uint32_t log_lde, uint32_t n_cols, int32_t from_monomials);
+/* bj_lde onto the cosets [coset_begin, coset_end) of the factor-2^log_lde domain only: d_out [col][coset_end - coset_begin][row],
+ * each coset bit-identical to its slot of the full bj_lde.  Unsharded contexts (BJ_ERR_UNSUPPORTED otherwise). */
+BJ_API int32_t bj_lde_cosets(bj_ctx* ctx, const uint64_t* d_in, uint64_t in_col_stride, uint64_t* d_out, uint32_t log_n, uint32_t log_lde,
+                             uint32_t coset_begin, uint32_t coset_end, uint32_t n_cols, int32_t from_monomials);
 
 /* ---- Poseidon2 Merkle tree: MerkleTreeWithCap::construct / construct_by_chunking /
  *      construct_by_chunking_from_flat_sources / continue_from_leaf_hashes (src/cs/oracle/merkle_tree.rs:78-449)
@@ -201,6 +214,11 @@ BJ_API int32_t bj_batch_inverse_ext(bj_ctx* ctx, uint64_t* d_c0, uint64_t* d_c1,
 BJ_API int32_t bj_deep_quotient_group(bj_ctx* ctx, const uint64_t* const* h_src_c0, const uint64_t* const* h_src_c1,
                                uint32_t n_src, const uint64_t* h_values_at, const uint64_t* h_challenges,
                                const uint64_t h_at[2], uint32_t log_rows, uint64_t* d_acc_c0, uint64_t* d_acc_c1);
+/* the same on the points [first_point, first_point + n_points) of the domain only: source columns and accumulators hold
+ * those n_points values (e.g. one coset recomputed by bj_lde_cosets, t = j * n + row).  Unsharded contexts. */
+BJ_API int32_t bj_deep_quotient_range(bj_ctx* ctx, const uint64_t* const* h_src_c0, const uint64_t* const* h_src_c1, uint32_t n_src,
+                                      const uint64_t* h_values_at, const uint64_t* h_challenges, const uint64_t h_at[2], uint32_t log_rows,
+                                      uint64_t first_point, uint64_t n_points, uint64_t* d_acc_c0, uint64_t* d_acc_c1);
 
 /* ---- stage 2, copy-permutation argument: compute_partial_products_in_extension
  *      (src/cs/implementations/copy_permutation.rs:649-766; rational :114-248, grand product :425-510) ----
@@ -469,6 +487,19 @@ typedef struct bj_proof bj_proof;
 BJ_API int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* d_sigmas, const uint64_t* d_constants,
                         const uint64_t* d_lookup_tables /* [lookup_width + 1][n] or NULL */, bj_setup** out);
 BJ_API void bj_setup_free(bj_setup* setup);
+/* Device bytes of bj_setup_create + bj_prove at their peak on each of `world` GPUs, counted from the circuit's shapes (host
+ * only, no device needed): out[0] the RESIDENT plan (every LDE column on all max(L, Q) cosets), out[1] the COMPACT plan (0
+ * when it does not apply: world > 1 or quotient degree >= LDE factor), which keeps cosets [0, Q) of the setup, witness and
+ * stage-2 columns after their trees are built and recomputes cosets [Q, L) from the natural-order columns for DEEP and the
+ * query answers.  Both are the context pool's allocations replayed in the driver's order plus an upper bound of what the
+ * library keeps outside the pool (twiddles, coset-power tables, NTT scratch). */
+BJ_API int32_t bj_proof_memory_plan(const bj_circuit* circuit, uint32_t world, uint64_t out[2]);
+/* 1 if bj_setup_create chose the compact plan, 0 if resident */
+BJ_API int32_t bj_setup_is_compact(const bj_setup* setup);
+/* the plan bj_setup_create chose: out[0] the peak bytes of the context's pool over bj_setup_create + bj_prove (what
+ * bj_ctx_memory_high_water reads on a fresh context), out[1] the bound on what the library holds outside the pool, out[2] the
+ * columns the compact plan recomputes at a time (0 on the resident plan) */
+BJ_API int32_t bj_setup_memory_plan(const bj_setup* setup, uint64_t out[3]);
 BJ_API int32_t bj_setup_get_cap(const bj_setup* setup, uint64_t* h_cap /* 4 * cap_size u64: VerificationKey::setup_merkle_tree_cap */);
 BJ_API int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables, const uint64_t* d_multiplicities /* or NULL */,
                  bj_proof** out);
