@@ -515,6 +515,36 @@ class Context:
                                                     self._ptr(out)))
         return out
 
+    # ---- satisfiability check (bj_check_satisfied / bj_lookup_multiplicities) ----
+    def check_if_satisfied(self, variables, sigmas, constants, gates, lookup=None):
+        """CSReferenceAssembly::check_if_satisfied (cs/implementations/satisfiability_test.rs:15-353) on the device: gates, copy
+        constraints (from sigma alone) and lookups of a witness, exactly.  variables / sigmas [V, n], constants [C, n],
+        lookup["tables"] [width + 1, n], lookup["multiplicities"] [n]: contiguous int64 CUDA tensors.  Returns the report as a
+        dict (bj_satisfiability_report without its padding); report["satisfied"] is 1 when nothing failed."""
+        for t in (variables, sigmas, constants) + ((lookup["tables"], lookup["multiplicities"]) if lookup else ()):
+            assert t.is_cuda and t.is_contiguous() and t.dtype == self._torch.int64
+        c, keep = _circuit(self, sigmas.shape[1].bit_length() - 1, sigmas.shape[0], constants.shape[0], gates, lookup)
+        rep = native.SatisfiabilityReport()
+        self._check(lib.bj_check_satisfied(self._h, ctypes.byref(c), self._ptr(sigmas), self._ptr(constants),
+                                           self._ptr(lookup["tables"]) if lookup else None, self._ptr(variables),
+                                           self._ptr(lookup["multiplicities"]) if lookup else None, ctypes.byref(rep)))
+        del keep
+        return rep.to_dict()
+
+    def materialize_multiplicities_polynomials(self, variables, constants, lookup):
+        """materialize_multiplicities_polynomials (cs/implementations/witness.rs:225-272) on the device: the lookup multiplicity
+        column [n] - on the first table row of every distinct content the number of tuples equal to it, 0 elsewhere.  Raises
+        BoojumError if a tuple matches no table row."""
+        for t in (variables, constants, lookup["tables"]):
+            assert t.is_cuda and t.is_contiguous() and t.dtype == self._torch.int64
+        n = variables.shape[1]
+        c, keep = _circuit(self, n.bit_length() - 1, variables.shape[0], constants.shape[0], [], lookup)
+        out = self._torch.empty(n, dtype=self._torch.int64, device=variables.device)
+        self._check(lib.bj_lookup_multiplicities(self._h, ctypes.byref(c), self._ptr(constants), self._ptr(lookup["tables"]),
+                                                 self._ptr(variables), self._ptr(out)))
+        del keep
+        return out
+
     # ---- native prover driver (bj_setup_create / bj_prove: host C++ inside the library) ----
     def native_setup(self, sigmas, constants, gates, quotient_degree, config, lookup=None, public_inputs=()):
         """bj_setup_create.  sigmas [V, n], constants [C, n], lookup["tables"] [width + 1, n]: contiguous int64 CUDA tensors
@@ -661,6 +691,18 @@ def proof_memory_plan(log_n, num_variables, num_constants, quotient_degree, conf
     return {"resident": int(out[0]), "compact": int(out[1]) or None}
 
 
+def _circuit(ctx, log_n, num_variables, num_constants, gates, lookup):
+    """bj_circuit with the trace shape, the gate programs and the lookup description filled in -> (circuit, keep-alive list)"""
+    keep, descs = ctx._gate_descs(gates)
+    c = native.Circuit()
+    c.log_n, c.num_variables, c.num_constants = log_n, num_variables, num_constants
+    c.gates, c.n_gates = descs, len(gates)
+    if lookup:
+        c.lookup_width, c.lookup_num_repetitions = lookup["width"], lookup["num_repetitions"]
+        c.lookup_variables_offset, c.lookup_table_id_column = lookup["variables_offset"], lookup["table_id_column"]
+    return c, keep
+
+
 class NativeSetup:
     """bj_setup: setup LDE + setup tree + circuit description held by the library; prove() runs bj_prove (host C++)."""
 
@@ -671,14 +713,9 @@ class NativeSetup:
         self._keep = [sigmas, constants, lookup["tables"] if lookup else None]
         for t in self._keep:
             assert t is None or (t.is_cuda and t.is_contiguous() and t.dtype == ctx._torch.int64)
-        keep, descs = ctx._gate_descs(gates)
-        c = native.Circuit()
-        c.log_n, c.num_variables, c.num_constants = sigmas.shape[1].bit_length() - 1, sigmas.shape[0], constants.shape[0]
+        c, keep = _circuit(ctx, sigmas.shape[1].bit_length() - 1, sigmas.shape[0], constants.shape[0], gates, lookup)
         c.quotient_degree, c.fri_lde_factor, c.merkle_tree_cap_size = quotient_degree, config.fri_lde_factor, config.merkle_tree_cap_size
-        c.security_level, c.pow_bits, c.gates, c.n_gates = config.security_level, config.pow_bits, descs, len(gates)
-        if lookup:
-            c.lookup_width, c.lookup_num_repetitions = lookup["width"], lookup["num_repetitions"]
-            c.lookup_variables_offset, c.lookup_table_id_column = lookup["variables_offset"], lookup["table_id_column"]
+        c.security_level, c.pow_bits = config.security_level, config.pow_bits
         pis = [(int(a), int(b)) for a, b in public_inputs]
         pc = (ctypes.c_uint32 * max(1, len(pis)))(*[a for a, _ in pis])
         pr = (ctypes.c_uint32 * max(1, len(pis)))(*[b for _, b in pis])

@@ -184,12 +184,24 @@ __device__ __forceinline__ void gate_step(u64 (&r)[K], const uint4* op, u32 stri
   GATE_CASE(OP, KIND_L, KIND_T) GATE_CASE(OP, KIND_L, KIND_L) GATE_CASE(OP, KIND_L, KIND_I)      \
   GATE_CASE(OP, KIND_I, KIND_T) GATE_CASE(OP, KIND_I, KIND_L) GATE_CASE(OP, KIND_I, KIND_I)
 
+// Check mode (bj_check_satisfied): the same interpreter on the trace domain, where every pushed term of a selected gate must be
+// 0.  A gate runs only where its selector is nonzero; per point the thread counts the (gate, repetition) instances with a
+// nonzero term and keeps the first one in (gate, repetition, term) order.  Each row belongs to one thread, so its first
+// failure is written to the row's slot without a race; the smallest (row, term index) key is found with atomicMin.
+struct GateCheckOut {
+  u64* first_value;              // [n_rows] the row's first nonzero term (written on failing rows only)
+  u64* first_selector;           // [n_rows] the selector of its gate
+  unsigned long long* failures;  // (row, gate, repetition) instances with a nonzero term
+  unsigned long long* first_key; // min of row << 32 | global term index (gate.term_base + rep * n_writes + term)
+};
+constexpr u32 GATE_NO_TERM = 0xffffffffu;
+
 // One thread owns K points (block b: points b * 128 * K + k * 128 + thread, so every column load is coalesced).  Decoding a
 // step costs the same for K points as for one (the one-point interpreter is bound by the instruction issue rate).  Tried and
 // dropped: fetching the next step's words ahead, a register budget of 128 with half the resident blocks, temporaries in
 // shared memory.
-template <int K, int S>
-__global__ void __launch_bounds__(128) gate_eval_kernel(const GateEvalParams p) {
+template <int K, int S, bool CHECK>
+__device__ __forceinline__ void gate_eval_body(const GateEvalParams& p, const GateCheckOut& chk) {
   u64 slots[S][K];
   const GateSlots<K> tmp{slots};
   const u64 first = (u64)blockIdx.x * (128 * K) + threadIdx.x;
@@ -199,13 +211,40 @@ __global__ void __launch_bounds__(128) gate_eval_kernel(const GateEvalParams p) 
   gl::e2 q[K];
 #pragma unroll
   for (int k = 0; k < K; k++) q[k] = {0, 0};
+  u32 fails[K], first_term[K];  // check mode: failing instances of the point, its first failing term (global index)
+  u64 first_val[K], first_sel[K];
+  if constexpr (CHECK) {
+#pragma unroll
+    for (int k = 0; k < K; k++) fails[k] = 0, first_term[k] = GATE_NO_TERM, first_val[k] = first_sel[k] = 0;
+  }
   for (u32 g = 0; g < p.n_gates; g++) {
     const DevGate gate = p.gates[g];
     gl::e2 acc[K];
 #pragma unroll
     for (int k = 0; k < K; k++) acc[k] = {0, 0};
-    if (gate.n_ops) {
+    u64 csel[K];  // check mode: the selector, known before the program runs
+    bool selected = true;
+    if constexpr (CHECK) {
+      selected = false;
+#pragma unroll
+      for (int k = 0; k < K; k++) {
+        u64 sel = 1;
+        for (u32 i = 0; i < gate.path_len; i++) {
+          const u64 c = gl::canon(__ldg(p.cols[p.consts_base + i] + pt[k]));
+          sel = gl::mul(sel, ((gate.path_bits >> i) & 1) ? c : gl::canon(gl::sub(1, c)));
+        }
+        csel[k] = gl::canon(sel);
+        selected |= csel[k] != 0;
+      }
+    }
+    if (gate.n_ops && selected) {
       for (u32 rep = 0; rep < gate.num_repetitions; rep++) {
+        u32 rep_term[K];  // check mode: smallest failing term index of this repetition (pushes come in program order)
+        u64 rep_val[K];
+        if constexpr (CHECK) {
+#pragma unroll
+          for (int k = 0; k < K; k++) rep_term[k] = GATE_NO_TERM, rep_val[k] = 0;
+        }
         const u64* alpha_rep = p.alphas + 2 * (size_t)(gate.term_base + rep * gate.n_writes);
         const uint4* op = reinterpret_cast<const uint4*>(p.ops + gate.ops_begin);
         for (u32 i = 0; i < gate.n_ops; i++, op += 2) {
@@ -251,43 +290,86 @@ __global__ void __launch_bounds__(128) gate_eval_kernel(const GateEvalParams p) 
               for (int k = 0; k < K; k++) r[k] = 0;
               break;
           }
-          if (w.x & 0x80u) {  // push_evaluation_result: the term times its alpha power goes into the gate's accumulator
-            const u64 a0 = __ldg(alpha_rep + 2 * dst), a1 = __ldg(alpha_rep + 2 * dst + 1);
+          if (w.x & 0x80u) {
+            if constexpr (CHECK) {  // the term must be 0 where the gate is selected
 #pragma unroll
-            for (int k = 0; k < K; k++) {
-              acc[k].c0 = gl::fma_lazy(r[k], a0, acc[k].c0);  // the running sum enters the 128-bit product before its one reduction
-              acc[k].c1 = gl::fma_lazy(r[k], a1, acc[k].c1);
+              for (int k = 0; k < K; k++) {
+                const u64 v = gl::canon(r[k]);
+                if (csel[k] != 0 && v != 0 && dst < rep_term[k]) rep_term[k] = dst, rep_val[k] = v;
+              }
+            } else {  // push_evaluation_result: the term times its alpha power goes into the gate's accumulator
+              const u64 a0 = __ldg(alpha_rep + 2 * dst), a1 = __ldg(alpha_rep + 2 * dst + 1);
+#pragma unroll
+              for (int k = 0; k < K; k++) {
+                acc[k].c0 = gl::fma_lazy(r[k], a0, acc[k].c0);  // the running sum enters the 128-bit product before its one reduction
+                acc[k].c1 = gl::fma_lazy(r[k], a1, acc[k].c1);
+              }
             }
           } else {
             tmp.store(dst, r);
           }
         }
+        if constexpr (CHECK) {
+#pragma unroll
+          for (int k = 0; k < K; k++) {
+            if (rep_term[k] == GATE_NO_TERM) continue;
+            fails[k]++;
+            if (first_term[k] == GATE_NO_TERM)
+              first_term[k] = gate.term_base + rep * gate.n_writes + rep_term[k], first_val[k] = rep_val[k], first_sel[k] = csel[k];
+          }
+        }
       }
     }
+    if constexpr (!CHECK) {
 #pragma unroll
-    for (int k = 0; k < K; k++) {
-      u64 sel = 1;
-      for (u32 i = 0; i < gate.path_len; i++) {
-        const u64 c = gl::canon(__ldg(p.cols[p.consts_base + i] + pt[k]));
-        sel = gl::mul(sel, ((gate.path_bits >> i) & 1) ? c : gl::canon(gl::sub(1, c)));
+      for (int k = 0; k < K; k++) {
+        u64 sel = 1;
+        for (u32 i = 0; i < gate.path_len; i++) {
+          const u64 c = gl::canon(__ldg(p.cols[p.consts_base + i] + pt[k]));
+          sel = gl::mul(sel, ((gate.path_bits >> i) & 1) ? c : gl::canon(gl::sub(1, c)));
+        }
+        q[k].c0 = gl::add(q[k].c0, gl::mul(acc[k].c0, sel));
+        q[k].c1 = gl::add(q[k].c1, gl::mul(acc[k].c1, sel));
       }
-      q[k].c0 = gl::add(q[k].c0, gl::mul(acc[k].c0, sel));
-      q[k].c1 = gl::add(q[k].c1, gl::mul(acc[k].c1, sel));
     }
   }
 #pragma unroll
   for (int k = 0; k < K; k++) {
     const u64 t = first + (u64)k * 128;
     if (t < p.n_rows) {
-      p.q_c0[t] = gl::canon(gl::add(p.q_c0[t], gl::canon(q[k].c0)));
-      p.q_c1[t] = gl::canon(gl::add(p.q_c1[t], gl::canon(q[k].c1)));
+      if constexpr (CHECK) {
+        if (fails[k]) {
+          atomicAdd(chk.failures, (unsigned long long)fails[k]);
+          chk.first_value[t] = first_val[k];
+          chk.first_selector[t] = first_sel[k];
+          atomicMin(chk.first_key, (unsigned long long)((t << 32) | first_term[k]));
+        }
+      } else {
+        p.q_c0[t] = gl::canon(gl::add(p.q_c0[t], gl::canon(q[k].c0)));
+        p.q_c1[t] = gl::canon(gl::add(p.q_c1[t], gl::canon(q[k].c1)));
+      }
     }
   }
 }
 
 template <int K, int S>
+__global__ void __launch_bounds__(128) gate_eval_kernel(const GateEvalParams p) {
+  gate_eval_body<K, S, false>(p, GateCheckOut{});
+}
+
+template <int K, int S>
+__global__ void __launch_bounds__(128) gate_check_kernel(const GateEvalParams p, const GateCheckOut chk) {
+  gate_eval_body<K, S, true>(p, chk);
+}
+
+template <int K, int S>
 static void gate_eval_launch(const GateEvalParams& p, cudaStream_t stream) {
   gate_eval_kernel<K, S><<<(unsigned)((p.n_rows + 128 * K - 1) / (128 * K)), 128, 0, stream>>>(p);
+}
+
+template <int K, int S>
+static void gate_check_launch(const GateEvalParams& p, const GateCheckOut& chk, cudaStream_t stream) {
+  gate_check_kernel<K, S><<<(unsigned)((p.n_rows + 128 * K - 1) / (128 * K)), 128, 0, stream>>>(p, chk);
 }
 
 }  // namespace bj
@@ -694,6 +776,53 @@ int32_t compile_gates(GateCompileError* err, int peephole, const bj_gate_desc* h
 }
 }  // namespace
 
+namespace bj {
+// K = 4 points per thread once there is enough work to fill the machine with such blocks
+static int gate_points_per_thread(const bj_ctx* ctx, u64 n_points) {
+  const int k = ctx->gate_points_per_thread;
+  if (k == 1 || k == 2 || k == 4) return k;
+  return n_points >= (u64)ctx->sm_count * 4 * 512 ? 4 : n_points >= (u64)ctx->sm_count * 4 * 256 ? 2 : 1;
+}
+
+struct GateProgramGuard {  // a long program's own buffer, freed (stream-ordered, i.e. after the kernel) on every exit path
+  void* p;
+  cudaStream_t s;
+  ~GateProgramGuard() {
+    if (p) cudaFreeAsync(p, s);
+  }
+};
+
+// gates, steps and the column table [variables | witnesses | constants] of a compiled program set -> p.gates, p.ops, p.cols,
+// p.consts_base.  Small programs ride in the parameter arena; a long one (the Poseidon2 flattened gate is ~9k relations) gets
+// its own stream-ordered buffer (*big_program: the caller's GateProgramGuard frees it, also when this fails)
+static int32_t gate_program_upload(bj_ctx* ctx, const CompiledGates& compiled, std::vector<const u64*> table, uint32_t consts_base,
+                                   GateEvalParams* p, void** big_program) {
+  const std::vector<PackedOp>& ops = compiled.ops;
+  void* d;
+  BJ_TRY(param_upload(ctx, compiled.gates.data(), sizeof(DevGate) * compiled.gates.size(), &d));
+  p->gates = (const DevGate*)d;
+  p->n_gates = (u32)compiled.gates.size();
+  static const PackedOp dummy_op{};
+  *big_program = nullptr;
+  const size_t ops_bytes = sizeof(PackedOp) * std::max<size_t>(ops.size(), 1);
+  if (ops_bytes > (128u << 10)) {
+    BJ_CUDA(ctx, cudaMallocAsync(big_program, ops_bytes, ctx->stream));
+    const cudaError_t e = cudaMemcpyAsync(*big_program, ops.data(), ops_bytes, cudaMemcpyHostToDevice, ctx->stream);
+    if (e != cudaSuccess)
+      BJ_FAIL(ctx, BJ_ERR_CUDA, std::string("gate program upload: ") + cudaGetErrorString(e));
+    d = *big_program;
+  } else {
+    BJ_TRY(param_upload(ctx, ops.empty() ? &dummy_op : ops.data(), ops_bytes, &d));
+  }
+  p->ops = (const PackedOp*)d;
+  if (table.empty()) table.push_back(nullptr);
+  BJ_TRY(param_upload(ctx, table.data(), sizeof(u64*) * table.size(), &d));
+  p->cols = (const u64* const*)d;
+  p->consts_base = consts_base;
+  return BJ_OK;
+}
+}  // namespace bj
+
 extern "C" int32_t bj_gate_programs_compile(const bj_gate_desc* h_gates, uint32_t n_gates, uint32_t n_variables, uint32_t n_witnesses,
                                             uint32_t n_constants, uint32_t peephole, uint64_t* h_records, uint64_t capacity_records,
                                             uint64_t* n_records, uint32_t* h_gate_first_record, uint32_t* max_live_temporaries) {
@@ -729,42 +858,13 @@ extern "C" int32_t bj_quotient_gates_general_purpose(bj_ctx* ctx, const bj_gate_
     const int32_t st = compile_gates(&err, ctx->gate_peephole, h_gates, n_gates, n_variables, n_witnesses, n_constants, compiled);
     if (st != BJ_OK) BJ_FAIL(ctx, st, err.last_error);
   }
-  std::vector<DevGate>& gates = compiled.gates;
-  std::vector<PackedOp>& ops = compiled.ops;
   const uint32_t max_slots = compiled.max_slots;
   const uint64_t total_terms = compiled.total_terms;
   if (total_terms > n_alpha_powers) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "not enough alpha powers for the gate terms");
   std::vector<u64> alphas(2 * (size_t)total_terms);
   for (size_t i = 0; i < alphas.size(); i++) alphas[i] = gl::canon(h_alpha_powers[i]);
   GateEvalParams p{};
-  void* d;
-  BJ_TRY(param_upload(ctx, gates.data(), sizeof(DevGate) * gates.size(), &d));
-  p.gates = (const DevGate*)d;
-  p.n_gates = n_gates;
-  static const PackedOp dummy_op{};
-  // small programs ride in the parameter arena; a long one (the Poseidon2 flattened gate is ~9k relations) gets its own
-  // stream-ordered buffer, released behind the kernel
-  void* big_program = nullptr;
-  const size_t ops_bytes = sizeof(PackedOp) * std::max<size_t>(ops.size(), 1);
-  if (ops_bytes > (128u << 10)) {
-    BJ_CUDA(ctx, cudaMallocAsync(&big_program, ops_bytes, ctx->stream));
-    const cudaError_t e = cudaMemcpyAsync(big_program, ops.data(), ops_bytes, cudaMemcpyHostToDevice, ctx->stream);
-    if (e != cudaSuccess) {
-      cudaFreeAsync(big_program, ctx->stream);
-      BJ_FAIL(ctx, BJ_ERR_CUDA, std::string("gate program upload: ") + cudaGetErrorString(e));
-    }
-    d = big_program;
-  } else {
-    BJ_TRY(param_upload(ctx, ops.empty() ? &dummy_op : ops.data(), ops_bytes, &d));
-  }
-  struct ProgramGuard {  // freed (stream-ordered, i.e. after the kernel) on every exit path
-    void* p;
-    cudaStream_t s;
-    ~ProgramGuard() {
-      if (p) cudaFreeAsync(p, s);
-    }
-  } program_guard{big_program, ctx->stream};
-  p.ops = (const PackedOp*)d;
+  GateProgramGuard program_guard{nullptr, ctx->stream};
   {
     std::vector<const u64*> table;
     table.reserve((size_t)n_variables + n_witnesses + n_constants + 1);
@@ -773,21 +873,17 @@ extern "C" int32_t bj_quotient_gates_general_purpose(bj_ctx* ctx, const bj_gate_
     for (uint32_t i = 0; i < n_constants; i++) table.push_back((const u64*)h_constant_cols[i]);
     for (const u64* c : table)
       if (!c) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_quotient_gates_general_purpose: NULL column");
-    if (table.empty()) table.push_back(nullptr);
-    BJ_TRY(param_upload(ctx, table.data(), sizeof(u64*) * table.size(), &d));
-    p.cols = (const u64* const*)d;
-    p.consts_base = n_variables + n_witnesses;
+    BJ_TRY(gate_program_upload(ctx, compiled, table, n_variables + n_witnesses, &p, &program_guard.p));
   }
+  void* d;
   static const u64 zero2[2] = {0, 0};
   BJ_TRY(param_upload(ctx, alphas.empty() ? (const void*)zero2 : (const void*)alphas.data(), sizeof(u64) * std::max<size_t>(alphas.size(), 2), &d));
   p.alphas = (const u64*)d;
   p.n_rows = n_points;
   p.q_c0 = (u64*)d_q_c0;
   p.q_c1 = (u64*)d_q_c1;
-  // K = 4 points per thread once there is enough work to fill the machine with such blocks; slots sized to the live maximum
-  // K = 4 points per thread once there is enough work to fill the machine with such blocks; slots sized to the live maximum
-  int k = ctx->gate_points_per_thread;
-  if (k != 1 && k != 2 && k != 4) k = n_points >= (u64)ctx->sm_count * 4 * 512 ? 4 : n_points >= (u64)ctx->sm_count * 4 * 256 ? 2 : 1;
+  // slots sized to the live maximum
+  const int k = gate_points_per_thread(ctx, n_points);
   const bool small = max_slots <= 32;
   if (k == 4) small ? gate_eval_launch<4, 32>(p, ctx->stream) : gate_eval_launch<4, GATE_MAX_TMP>(p, ctx->stream);
   else if (k == 2) small ? gate_eval_launch<2, 32>(p, ctx->stream) : gate_eval_launch<2, GATE_MAX_TMP>(p, ctx->stream);

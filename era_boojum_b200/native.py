@@ -133,6 +133,8 @@ SIGNATURES = {
     "bj_proof_free": (None, [_vp]),
     "bj_proof_to_json": (_i32, [_vp, _vp, _sz, ctypes.POINTER(_sz)]),
     "bj_proof_stage_seconds": (_i32, [_vp, _vp]),
+    "bj_check_satisfied": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bj_lookup_multiplicities": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp]),
     "bj_selftest_field": (_i32, [_vp, _u64, _u64, _vp]),
     "bj_host_gl_mul": (_u64, [_u64, _u64]),
     "bj_host_gl_add": (_u64, [_u64, _u64]),
@@ -186,3 +188,27 @@ class Circuit(ctypes.Structure):
                 ("lookup_variables_offset", ctypes.c_uint32), ("lookup_table_id_column", ctypes.c_uint32),
                 ("public_input_columns", ctypes.POINTER(ctypes.c_uint32)), ("public_input_rows", ctypes.POINTER(ctypes.c_uint32)),
                 ("n_public_inputs", ctypes.c_uint32), ("tree_hasher", ctypes.c_uint32), ("transcript", ctypes.c_uint32)]
+
+
+SIGMA_NO_CELL, SIGMA_UNNAMED, SIGMA_NAMED_TWICE = 1, 2, 3
+
+
+class SatisfiabilityReport(ctypes.Structure):
+    """bj_satisfiability_report"""
+    _fields_ = [("satisfied", ctypes.c_uint32), ("reserved0", ctypes.c_uint32),
+                ("gate_failures", ctypes.c_uint64), ("gate_row", ctypes.c_uint64), ("gate_index", ctypes.c_uint32),
+                ("gate_repetition", ctypes.c_uint32), ("gate_term", ctypes.c_uint32), ("reserved1", ctypes.c_uint32),
+                ("gate_value", ctypes.c_uint64), ("gate_selector", ctypes.c_uint64),
+                ("copy_failures", ctypes.c_uint64), ("copy_row", ctypes.c_uint64), ("copy_other_row", ctypes.c_uint64),
+                ("copy_column", ctypes.c_uint32), ("copy_other_column", ctypes.c_uint32),
+                ("copy_value", ctypes.c_uint64), ("copy_other_value", ctypes.c_uint64),
+                ("sigma_failures", ctypes.c_uint64), ("sigma_row", ctypes.c_uint64), ("sigma_column", ctypes.c_uint32),
+                ("sigma_kind", ctypes.c_uint32),
+                ("lookup_unmatched", ctypes.c_uint64), ("lookup_row", ctypes.c_uint64), ("lookup_subargument", ctypes.c_uint32),
+                ("reserved2", ctypes.c_uint32),
+                ("multiplicity_failures", ctypes.c_uint64), ("multiplicity_row", ctypes.c_uint64),
+                ("multiplicity_count", ctypes.c_uint64), ("multiplicity_sum", ctypes.c_uint64)]
+
+    def to_dict(self):
+        """the report without its padding fields"""
+        return {name: int(getattr(self, name)) for name, _ in self._fields_ if not name.startswith("reserved")}

@@ -510,6 +510,75 @@ BJ_API int32_t bj_proof_to_json(const bj_proof* proof, char* buf, size_t capacit
 /* wall-clock seconds of the six stages (witness, stage 2, quotient, openings, DEEP+FRI, queries), device work included */
 BJ_API int32_t bj_proof_stage_seconds(const bj_proof* proof, double out[6]);
 
+/* ---- satisfiability check: CSReferenceAssembly::check_if_satisfied (src/cs/implementations/satisfiability_test.rs:15-353) ----
+ * Checks a witness against its circuit exactly (no random challenge) on the trace domain, from the natural-order device columns
+ * bj_setup_create and bj_prove take, with no setup (no LDE, no tree).  It reads log_n, num_variables, num_constants,
+ * gates / n_gates and the lookup_* fields of the circuit and ignores the rest.  Three conditions, the ones bj_prove needs:
+ *   - gates: every pushed term of every repetition of every gate is 0 on every row where the gate's selector (the product along
+ *     its path over constant columns 0 .. path_len - 1) is nonzero; gates on specialised columns have no selector and run on
+ *     every row;
+ *   - copy constraints, from sigma alone: the entry s = k_c' w^r' of cell (c, r) names cell (c', r') (c' from s^n = k_c'^n, r'
+ *     the discrete log of s / k_c' in <w_n>); each cell holds the value of the cell it names, and sigma is well formed: every
+ *     entry names a cell (BJ_SIGMA_NO_CELL) and every cell is named by exactly one entry (BJ_SIGMA_UNNAMED, BJ_SIGMA_NAMED_TWICE);
+ *   - lookups (lookup_width > 0): every tuple (the row's lookup_width columns of a sub-argument, then the table id from constant
+ *     column lookup_table_id_column) equals a row of the table columns [lookup_width + 1][n] (id last), and for every distinct
+ *     table content the number of tuples equal to it is the sum mod p of d_multiplicities over the table rows with that content.
+ * Values are compared canonically (x + p equals x).  Returns BJ_OK whether or not the witness is satisfied (the report says
+ * which); BJ_ERR_INVALID_ARG, with a message and no kernel launched, for malformed arguments: NULL columns, lookup_width > 0
+ * without tables or multiplicities, a table-id column out of range, a lookup shape bj_prove refuses (more than 32
+ * sub-arguments or 7 columns per tuple), gate programs the gate compiler rejects.  Synchronises.  Never communicates: it runs
+ * the same on a sharded context.
+ * Scratch from the context's pool, released before it returns: 16 n (gates) + 24 n (powers of w) + V n / 4 (two bitmaps) +
+ * 24 V + 32 n (lookups) bytes, n = 2^log_n, V = num_variables - e.g. 72 n + V n / 4 bytes, about 400 MB at n = 2^22, V = 92.
+ * Every count and "first" field is deterministic.  A "first" field is 0 when its count is 0. */
+#define BJ_SIGMA_NO_CELL 1u      /* the cell's sigma entry is not k_c w^r for any column c < num_variables and row r */
+#define BJ_SIGMA_UNNAMED 2u      /* no sigma entry names the cell */
+#define BJ_SIGMA_NAMED_TWICE 3u  /* two or more sigma entries name the cell */
+typedef struct bj_satisfiability_report {
+  uint32_t satisfied; /* 1 if every count below is 0 */
+  uint32_t reserved0;
+  /* gates: (row, gate, repetition) instances with a nonzero term; the first in (row, gate, repetition, term) order */
+  uint64_t gate_failures;
+  uint64_t gate_row;
+  uint32_t gate_index;      /* into circuit->gates */
+  uint32_t gate_repetition;
+  uint32_t gate_term;       /* index into the gate's writes */
+  uint32_t reserved1;
+  uint64_t gate_value;      /* the term's value (canonical) */
+  uint64_t gate_selector;   /* the gate's selector on that row */
+  /* copy constraints: cells whose value differs from the cell their sigma entry names; the first in (row, column) order */
+  uint64_t copy_failures;
+  uint64_t copy_row, copy_other_row;
+  uint32_t copy_column, copy_other_column;
+  uint64_t copy_value, copy_other_value;
+  /* malformed sigma: entries naming no cell + cells named by no entry + cells named more than once; the first in
+   * (row, column, kind) order */
+  uint64_t sigma_failures;
+  uint64_t sigma_row;
+  uint32_t sigma_column;
+  uint32_t sigma_kind;      /* BJ_SIGMA_* */
+  /* lookups: tuples that match no table row, the first in (row, sub-argument) order */
+  uint64_t lookup_unmatched;
+  uint64_t lookup_row;
+  uint32_t lookup_subargument;
+  uint32_t reserved2;
+  /* distinct table contents whose tuple count is not their multiplicity sum, the first by its first table row */
+  uint64_t multiplicity_failures;
+  uint64_t multiplicity_row;
+  uint64_t multiplicity_count; /* tuples equal to the content */
+  uint64_t multiplicity_sum;   /* sum mod p of d_multiplicities over the rows with that content */
+} bj_satisfiability_report;
+BJ_API int32_t bj_check_satisfied(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* d_sigmas, const uint64_t* d_constants,
+                                  const uint64_t* d_lookup_tables /* or NULL */, const uint64_t* d_variables,
+                                  const uint64_t* d_multiplicities /* or NULL */, bj_satisfiability_report* out);
+/* materialize_multiplicities_polynomials (src/cs/implementations/witness.rs:225-272) on the device: d_multiplicities (n values)
+ * receives, on the first table row of every distinct content, the number of lookup tuples equal to it, and 0 on every other
+ * row.  The circuit fields read and the argument rules are those of bj_check_satisfied; the circuit must have a lookup
+ * argument.  BJ_ERR_INVALID_ARG, naming the first such tuple, if a tuple matches no table row (no valid column exists then).
+ * Scratch: 16 n bytes.  Synchronises. */
+BJ_API int32_t bj_lookup_multiplicities(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* d_constants, const uint64_t* d_lookup_tables,
+                                        const uint64_t* d_variables, uint64_t* d_multiplicities /* out: n values */);
+
 /* device self-test: PTX field arithmetic vs the portable C versions on n pseudo-random + edge inputs */
 BJ_API int32_t bj_selftest_field(bj_ctx* ctx, uint64_t n, uint64_t seed, uint64_t* h_mismatches);
 
