@@ -242,8 +242,9 @@ class Context:
 
     def set_memory_limit(self, nbytes):
         """bj_ctx_set_memory_limit: device bytes a proof on this context may use (0: what is free when the setup is created).
-        native_setup picks the resident plan if it fits, the compact one otherwise, and raises BoojumError (out of device
-        memory, with both plans' byte counts) if neither does."""
+        native_setup picks the resident plan if it fits, else the compact one (quotient degree < LDE factor), else the streamed
+        one (quotient degree > LDE factor), and raises BoojumError (out of device memory, with every applicable plan's byte
+        count) if none does."""
         self._check(lib.bj_ctx_set_memory_limit(self._h, int(nbytes)))
 
     def memory_high_water(self, reset=False):
@@ -679,7 +680,9 @@ class Comm:
 
 def proof_memory_plan(log_n, num_variables, num_constants, quotient_degree, config, lookup=None, world=1):
     """bj_proof_memory_plan: device bytes of native_setup + prove at their peak on each of `world` GPUs, counted from the
-    shapes (no device needed).  -> dict(resident=bytes, compact=bytes or None when the compact plan does not apply)."""
+    shapes (no device needed).  -> dict(resident=bytes, compact=bytes or None, streamed=bytes or None), None where the plan
+    does not apply (compact: one GPU with quotient degree < LDE factor; streamed: one GPU with quotient degree > LDE factor,
+    bj_proof_memory_plan_streamed)."""
     c = native.Circuit()
     c.log_n, c.num_variables, c.num_constants, c.quotient_degree = log_n, num_variables, num_constants, quotient_degree
     c.fri_lde_factor, c.merkle_tree_cap_size = config.fri_lde_factor, config.merkle_tree_cap_size
@@ -688,7 +691,9 @@ def proof_memory_plan(log_n, num_variables, num_constants, quotient_degree, conf
         c.lookup_width, c.lookup_num_repetitions = lookup["width"], lookup["num_repetitions"]
     out = (ctypes.c_uint64 * 2)()
     _ok(lib.bj_proof_memory_plan(ctypes.byref(c), world, out), "bj_proof_memory_plan")
-    return {"resident": int(out[0]), "compact": int(out[1]) or None}
+    streamed = ctypes.c_uint64()
+    _ok(lib.bj_proof_memory_plan_streamed(ctypes.byref(c), world, ctypes.byref(streamed)), "bj_proof_memory_plan_streamed")
+    return {"resident": int(out[0]), "compact": int(out[1]) or None, "streamed": int(streamed.value) or None}
 
 
 def _circuit(ctx, log_n, num_variables, num_constants, gates, lookup):
@@ -734,6 +739,13 @@ class NativeSetup:
     def compact(self):
         """True if bj_setup_create chose the compact memory plan"""
         return lib.bj_setup_is_compact(self._h) == 1
+
+    @property
+    def plan(self):
+        """the memory plan bj_setup_create chose (bj_setup_plan): "resident", "compact" or "streamed\""""
+        k = lib.bj_setup_plan(self._h)
+        _ok(min(k, 0), "bj_setup_plan")
+        return {native.PLAN_RESIDENT: "resident", native.PLAN_COMPACT: "compact", native.PLAN_STREAMED: "streamed"}[k]
 
     def memory_plan(self):
         """bj_setup_memory_plan: the chosen plan -> dict(pool=peak pool bytes of setup + prove, outside_pool=bound on the

@@ -73,6 +73,15 @@ struct CosetShard {
     if (log_split) s = gl::mul(s, gl::pow(gl::omega(log_n), pr));
     return s;
   }
+  // the window of one coset j of 2^log_cosets: a buffer that holds coset j alone is the local layout of rank j in a coset
+  // shard of world 2^log_cosets, so the row-local kernels reading it get global_index(t) = j * n + t, the coset's x(t) and
+  // vanishing constant, and z(omega x) inside the same coset, exactly as on the whole domain
+  __host__ static CosetShard window(uint32_t log_cosets, uint32_t j) {
+    CosetShard w;
+    w.first = j;
+    w.log_stride = log_cosets;
+    return w;
+  }
 };
 
 }  // namespace bj

@@ -181,6 +181,24 @@ static int32_t keep_first_cosets_grouped(bj_ctx* ctx, ColumnGroups& g, std::vect
   return BJ_OK;
 }
 
+// the LDE columns a plan keeps: every coset of the factor-2^log_d domain (lde_columns), or on the streamed plan only the
+// first `streamed_cosets` = L, stride n * L (bj_lde_cosets: the same coset transforms, so the values are bit-identical)
+static int32_t lde_kept(bj_ctx* ctx, const uint64_t* d_in, uint64_t* d_out, u32 log_n, u32 log_d, u32 n_cols, u32 streamed_cosets) {
+  if (!streamed_cosets) return lde_columns(ctx, d_in, d_out, log_n, log_d, n_cols);
+  return n_cols ? bj_lde_cosets(ctx, d_in, 1ull << log_n, d_out, log_n, log_d, 0, streamed_cosets, n_cols, 0) : BJ_OK;
+}
+
+// streamed plan: while the quotient kernels of coset j run on a buffer that holds coset j alone, the context's shard is
+// the window of coset j; the caller's shard comes back on every exit path
+struct ShardWindow {
+  bj_ctx* ctx;
+  CosetShard saved;
+  ShardWindow(bj_ctx* c, u32 log_cosets, u32 j) : ctx(c), saved(c->shard) { c->shard = CosetShard::window(log_cosets, j); }
+  ~ShardWindow() { ctx->shard = saved; }
+  ShardWindow(const ShardWindow&) = delete;
+  ShardWindow& operator=(const ShardWindow&) = delete;
+};
+
 int32_t copy_permutation_stage2_sharded(bj_ctx* ctx, const uint64_t* const* h_variable_cols, const uint64_t* const* h_sigma_cols, u32 n_cols,
                                         const uint64_t* h_non_residues, gl::e2 beta, gl::e2 gamma, u32 log_n, u32 chunk_size, u64* d_out);  // stage2.cu
 
@@ -245,18 +263,22 @@ struct QueryAnswer {
 };
 
 // ---- memory plan: the one owner of what bj_setup_create + bj_prove hold on the device at their peak ----
-// Two plans.  RESIDENT keeps every LDE column on all D = max(L, Q) cosets until the proof is done.  COMPACT (one GPU, Q < L)
+// Three plans.  RESIDENT keeps every LDE column on all D = max(L, Q) cosets until the proof is done.  COMPACT (one GPU, Q < L)
 // keeps only the first Q cosets of the setup, witness and stage-2 columns once their trees are built: the quotient reads
 // cosets [0, Q) and the openings coset 0, so cosets [Q, L) are read by DEEP and the query answers only, and those two
 // recompute them from the natural-order columns, a chunk of columns and one coset at a time.  The quotient oracle stays
-// resident.  The plan replays the driver's stream-ordered pool allocations in order (pool_peak) and adds what the library
-// keeps outside the pool (library_reserve): twiddles, coset-power tables and the NTT scratch.
+// resident.  STREAMED (one GPU, Q > L) evaluates the setup, witness and stage-2 columns on the committed cosets [0, L) only:
+// cosets [L, Q) are read by the quotient alone, which evaluates every column it reads onto one such coset at a time into a
+// coset-sized scratch, from the natural-order columns (the stage-2 ones are kept for it).  The plan replays the driver's
+// stream-ordered pool allocations in order (pool_peak) and adds what the library keeps outside the pool (library_reserve):
+// twiddles, coset-power tables and the NTT scratch.
+enum MemoryPlan : u32 { PLAN_RESIDENT = BJ_PLAN_RESIDENT, PLAN_COMPACT = BJ_PLAN_COMPACT, PLAN_STREAMED = BJ_PLAN_STREAMED };
 struct ProofShape {
   u32 V, C, T, W, n_s2, Q, L, log_n, log_l, log_d, log_q, world, split, cap, n_queries, sched_len;
   u32 sched[32];
   u64 n;
   bool lk;
-  u32 nat_cols() const { return V + C + T + W + n_s2; }  // natural-order columns a compact proof recomputes from
+  u32 nat_cols() const { return V + C + T + W + n_s2; }  // natural-order columns a compact / streamed proof recomputes from
 };
 
 static int32_t proof_shape(const bj_circuit& c, u32 world, ProofShape* s) {
@@ -296,9 +318,11 @@ struct Ledger {
 };
 
 // peak pool bytes of bj_setup_create followed by bj_prove; `chunk`: columns recomputed at a time (compact plan)
-static u64 pool_peak(const ProofShape& s, bool compact, u32 chunk) {
+static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk) {
   Ledger m;
-  const u64 n = s.n, w = s.world, nD = (n << s.log_d) / w, nL = (n << s.log_l) / w, nQ = n << s.log_q, Qn = n * s.Q;
+  const bool compact = plan == PLAN_COMPACT, streamed = plan == PLAN_STREAMED;
+  const u64 n = s.n, w = s.world, nL = (n << s.log_l) / w, nQ = n << s.log_q, Qn = n * s.Q;
+  const u64 nD = streamed ? nL : (n << s.log_d) / w;  // elements of an LDE column as first evaluated
   const u64 leaves = (n << s.log_l) / w, capl = s.cap / w;
   auto tree = [&]() {
     m.add(4 * leaves);
@@ -354,7 +378,8 @@ static u64 pool_peak(const ProofShape& s, bool compact, u32 chunk) {
   }
   const u64 zn = s.split ? 2 * nD : 0;
   if (zn) m.add(zn);
-  if (!compact) m.sub(s.n_s2 * n);  // the compact plan keeps the natural stage-2 columns for DEEP and the queries
+  // the compact plan keeps the natural stage-2 columns for DEEP and the queries, the streamed plan for the quotient
+  if (!compact && !streamed) m.sub(s.n_s2 * n);
   tree();
   if (compact)
     for (u64 g : sg) {
@@ -363,6 +388,10 @@ static u64 pool_peak(const ProofShape& s, bool compact, u32 chunk) {
     }
   // round 3
   m.add(2 * nQ);
+  if (streamed) {  // one coset of every column the quotient reads
+    m.add((u64)s.nat_cols() * n);
+    m.sub((u64)s.nat_cols() * n);
+  }
   const u64 nQl = ((u64)s.Q << s.split) >= w ? nQ / w : n >> s.split;
   if (w > 1) m.add(2 * std::max<u64>(nQl, 1));
   if (zn) m.sub(zn);
@@ -438,8 +467,9 @@ static u64 library_reserve(const ProofShape& s) {
 }
 
 static bool compact_applies(const ProofShape& s) { return s.world == 1 && s.Q < s.L; }
+static bool streamed_applies(const ProofShape& s) { return s.world == 1 && s.Q > s.L; }
 
-static u64 plan_bytes(const ProofShape& s, bool compact, u32 chunk = 2) { return pool_peak(s, compact, chunk) + library_reserve(s); }
+static u64 plan_bytes(const ProofShape& s, MemoryPlan plan, u32 chunk = 2) { return pool_peak(s, plan, chunk) + library_reserve(s); }
 
 }  // namespace bj
 
@@ -453,10 +483,11 @@ struct bj_setup {
   uint32_t n_tables = 0;
   bj::DevMem lde;  // [V + C + T][D][n], D = max(L, quotient degree): the tree commits to the first L cosets of every column
   bj::Oracle tree;
-  uint64_t col_len = 0;  // elements of one LDE column held by this context: n * (D / world), or n * Q on the compact plan
-  bool compact = false;  // memory plan chosen by bj_setup_create, followed by bj_prove
+  uint64_t col_len = 0;  // elements of one LDE column held by this context: n * (D / world), n * Q compact, n * L streamed
+  bool compact = false;   // memory plan chosen by bj_setup_create, followed by bj_prove
+  bool streamed = false;
   uint64_t limit = 0;    // the device-memory limit the plan was chosen under
-  uint64_t plan[2] = {0, 0};  // resident, compact (0: no compact plan)
+  uint64_t plan[3] = {0, 0, 0};  // resident, compact, streamed (0: the plan does not apply)
   uint32_t chunk = 2;         // compact plan: natural-order columns recomputed at a time
   uint64_t pool_bytes = 0, outside_pool_bytes = 0;  // the chosen plan (with its chunk): pool peak, library reserve
   uint64_t chosen_bytes() const { return pool_bytes + outside_pool_bytes; }
@@ -513,9 +544,10 @@ static int32_t memory_limit(bj_ctx* ctx, uint64_t* out) {
   return BJ_OK;
 }
 
-static std::string plan_message(const char* who, const uint64_t plan[2], uint64_t limit) {
+static std::string plan_message(const char* who, const uint64_t plan[3], uint64_t limit) {
   std::string m = std::string(who) + ": the proof needs " + std::to_string(plan[0]) + " bytes of device memory resident";
   m += plan[1] ? " and " + std::to_string(plan[1]) + " bytes on the compact plan" : std::string(" (no compact plan: sharded context or quotient degree >= LDE factor)");
+  if (plan[2]) m += " and " + std::to_string(plan[2]) + " bytes on the streamed plan";
   return m + ", above the limit of " + std::to_string(limit) + " bytes";
 }
 
@@ -563,13 +595,17 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
   }
   std::unique_ptr<bj_setup> s(new bj_setup());
   {
-    // the memory plan: resident if it fits under the limit, compact otherwise; refused before anything is launched
+    // the memory plan: resident if it fits under the limit, else compact (Q < L), else streamed (Q > L); refused before
+    // anything is launched
     ProofShape sh;
     BJ_TRY(proof_shape(*circuit, comm_world(ctx), &sh));
-    s->plan[0] = plan_bytes(sh, false);
-    s->plan[1] = compact_applies(sh) ? plan_bytes(sh, true) : 0;
+    s->plan[0] = plan_bytes(sh, PLAN_RESIDENT);
+    s->plan[1] = compact_applies(sh) ? plan_bytes(sh, PLAN_COMPACT) : 0;
+    s->plan[2] = streamed_applies(sh) ? plan_bytes(sh, PLAN_STREAMED) : 0;
     BJ_TRY(memory_limit(ctx, &s->limit));
-    if (s->plan[0] > s->limit) {
+    if (s->plan[0] > s->limit && s->plan[2] && s->plan[2] <= s->limit) {
+      s->streamed = true;
+    } else if (s->plan[0] > s->limit) {
       if (!s->plan[1] || s->plan[1] > s->limit) BJ_FAIL(ctx, BJ_ERR_OOM, plan_message("bj_setup_create", s->plan, s->limit));
       s->compact = true;
       // wider recompute chunks only save kernel launches: the chunk grows into at most half of the headroom the limit leaves
@@ -578,12 +614,12 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
       uint32_t lo = 2, hi = std::max<uint32_t>(2, std::min<uint32_t>(16, sh.nat_cols()));
       while (lo < hi) {
         const uint32_t mid = lo + (hi - lo + 1) / 2;
-        if (plan_bytes(sh, true, mid) <= budget) lo = mid;
+        if (plan_bytes(sh, PLAN_COMPACT, mid) <= budget) lo = mid;
         else hi = mid - 1;
       }
       s->chunk = lo;
     }
-    s->pool_bytes = pool_peak(sh, s->compact, s->chunk);
+    s->pool_bytes = pool_peak(sh, s->compact ? PLAN_COMPACT : s->streamed ? PLAN_STREAMED : PLAN_RESIDENT, s->chunk);
     s->outside_pool_bytes = library_reserve(sh);
   }
   s->ctx = ctx;
@@ -620,11 +656,14 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
   const uint32_t V = circuit->num_variables, C = circuit->num_constants, T = s->n_tables;
   const uint32_t log_n = circuit->log_n, log_l = s->log_l(), log_d = s->log_d();
   const u64 n = 1ull << log_n;
-  s->col_len = (n << log_d) / comm_world(ctx);
+  // the streamed plan evaluates the committed cosets [0, L) only; the quotient recomputes the others from the borrowed
+  // natural-order columns
+  const uint32_t kept = s->streamed ? circuit->fri_lde_factor : 0;
+  s->col_len = s->streamed ? n << log_l : (n << log_d) / comm_world(ctx);
   BJ_TRY(s->lde.alloc(ctx, (size_t)(V + C + T) * s->col_len));
-  BJ_TRY(lde_columns(ctx, d_sigmas, (uint64_t*)s->lde.p, log_n, log_d, V));
-  if (C) BJ_TRY(lde_columns(ctx, d_constants, (uint64_t*)s->lde.p + (size_t)V * s->col_len, log_n, log_d, C));
-  if (T) BJ_TRY(lde_columns(ctx, d_lookup_tables, (uint64_t*)s->lde.p + (size_t)(V + C) * s->col_len, log_n, log_d, T));
+  BJ_TRY(lde_kept(ctx, d_sigmas, (uint64_t*)s->lde.p, log_n, log_d, V, kept));
+  if (C) BJ_TRY(lde_kept(ctx, d_constants, (uint64_t*)s->lde.p + (size_t)V * s->col_len, log_n, log_d, C, kept));
+  if (T) BJ_TRY(lde_kept(ctx, d_lookup_tables, (uint64_t*)s->lde.p + (size_t)(V + C) * s->col_len, log_n, log_d, T, kept));
   for (uint32_t j = 0; j < V + C + T; j++) s->tree.cols.push_back(s->col(j));
   BJ_TRY(oracle_build(ctx, s->tree, n << log_l, circuit->merkle_tree_cap_size, circuit->tree_hasher, circuit->fri_lde_factor));
   if (s->compact) {
@@ -672,9 +711,11 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   const u64 nQl = ctx->shard.local_points(Q, (int)log_n);                 // LOCAL quotient points
   const uint32_t split = ctx->shard.log_split;                            // 2^split row blocks per coset (split domain shard)
   const u64 nb = n >> split;                                             // rows of one unit
-  const bool compact = setup->compact;
+  const bool compact = setup->compact, streamed = setup->streamed;
   const u64 Qn = n * Q;  // compact plan: elements of a setup / witness / stage-2 column kept on the device (cosets [0, Q))
-  if (setup->col_len != (compact ? Qn : nD)) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: the setup was built with a different shard");
+  const uint32_t kept = streamed ? L : 0;  // streamed plan: those columns are evaluated on the cosets [0, L) only
+  const u64 nK = streamed ? nL : nD;      // stride of those columns on the resident and streamed plans
+  if (setup->col_len != (compact ? Qn : nK)) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: the setup was built with a different shard");
   const uint32_t chunk = setup->chunk;  // compact plan: natural-order columns recomputed at a time
   {
     const uint64_t limit = ctx->memory_limit ? ctx->memory_limit : setup->limit;
@@ -726,12 +767,12 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     BJ_TRY(lde_grouped(ctx, w_groups, d_variables, V, log_n, log_d, w_cols.data()));
     if (lk) BJ_TRY(lde_grouped(ctx, w_groups, d_multiplicities, 1, log_n, log_d, &m_col));
   } else {
-    BJ_TRY(w_lde.alloc(ctx, (size_t)V * nD));
-    BJ_TRY(lde_columns(ctx, d_variables, (uint64_t*)w_lde.p, log_n, log_d, V));
-    for (uint32_t j = 0; j < V; j++) w_cols[j] = (const uint64_t*)w_lde.p + (size_t)j * nD;
+    BJ_TRY(w_lde.alloc(ctx, (size_t)V * nK));
+    BJ_TRY(lde_kept(ctx, d_variables, (uint64_t*)w_lde.p, log_n, log_d, V, kept));
+    for (uint32_t j = 0; j < V; j++) w_cols[j] = (const uint64_t*)w_lde.p + (size_t)j * nK;
     if (lk) {
-      BJ_TRY(m_lde.alloc(ctx, nD));
-      BJ_TRY(bj_lde(ctx, d_multiplicities, n, (uint64_t*)m_lde.p, log_n, log_d, 1, 0));
+      BJ_TRY(m_lde.alloc(ctx, nK));
+      BJ_TRY(lde_kept(ctx, d_multiplicities, (uint64_t*)m_lde.p, log_n, log_d, 1, kept));
       m_col = (const uint64_t*)m_lde.p;
     }
   }
@@ -787,9 +828,9 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   if (compact) {
     BJ_TRY(lde_grouped(ctx, s2_groups, (const uint64_t*)st2.p, n_s2, log_n, log_d, s2_cols.data()));
   } else {
-    BJ_TRY(s2_lde.alloc(ctx, (size_t)n_s2 * nD));
-    BJ_TRY(lde_columns(ctx, (const uint64_t*)st2.p, (uint64_t*)s2_lde.p, log_n, log_d, n_s2));
-    for (uint32_t j = 0; j < n_s2; j++) s2_cols[j] = (const uint64_t*)s2_lde.p + (size_t)j * nD;
+    BJ_TRY(s2_lde.alloc(ctx, (size_t)n_s2 * nK));
+    BJ_TRY(lde_kept(ctx, (const uint64_t*)st2.p, (uint64_t*)s2_lde.p, log_n, log_d, n_s2, kept));
+    for (uint32_t j = 0; j < n_s2; j++) s2_cols[j] = (const uint64_t*)s2_lde.p + (size_t)j * nK;
   }
   // a row block of a split shard does not hold z(omega x) (another block of the coset does).  On a unit with shift sigma,
   // z(omega x) is the LDE of z on the shift sigma * omega in the same row order: two more columns (c0, c1 of z)
@@ -798,7 +839,7 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     BJ_TRY(z_next.alloc(ctx, 2 * nD));
     BJ_TRY(bj_lde_next_row(ctx, (const uint64_t*)st2.p, n, (uint64_t*)z_next.p, log_n, log_d, 2, 0));
   }
-  if (!compact) st2.release();  // the compact plan recomputes cosets [Q, L) of stage 2 from it
+  if (!compact && !streamed) st2.release();  // the compact plan recomputes cosets [Q, L) of stage 2 from it, the streamed [L, Q)
   Oracle s2_or;
   s2_or.cols = s2_cols;
   BJ_TRY(oracle_build(ctx, s2_or, n << log_l, cap, c.tree_hasher, L));
@@ -844,34 +885,74 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   } else {
     BJ_CUDA(ctx, cudaMemsetAsync(qq.p, 0, sizeof(u64) * 2 * nQ, ctx->stream));
   }
-  if (nQl) {
-  if (lk) {
-    std::vector<const uint64_t*> ll(wdt * nsub), al(2 * nsub);
-    for (uint32_t i = 0; i < wdt * nsub; i++) ll[i] = w_cols[voff + i];
-    for (uint32_t i = 0; i < 2 * nsub; i++) al[i] = s2_cols[a_off + i];
-    const uint64_t lb[2] = {lookup_beta.c0, lookup_beta.c1}, lg[2] = {lookup_gamma.c0, lookup_gamma.c1};
-    BJ_TRY(bj_quotient_lookup_specialized(ctx, ll.data(), nsub, wdt, const_cols[c.lookup_table_id_column], table_cols.data(), T,
-                                          m_col, al.data(), s2_cols[a_off + 2 * nsub], s2_cols[a_off + 2 * nsub + 1], lb, lg,
-                                          powers.data(), nQl, q0, q1));
+  // the quotient's terms and the division by the vanishing polynomial on the n_points points the context's shard reads, from
+  // the LDE columns of what the quotient reads (variables, multiplicities, sigmas, constants, tables, stage 2)
+  struct QuotientCols {
+    std::vector<const uint64_t*> w, sigma, consts, tables, s2;
+    const uint64_t* m;
+  };
+  auto quotient_terms = [&](const QuotientCols& k, u64 n_points, uint64_t* o0, uint64_t* o1) -> int32_t {
+    if (lk) {
+      std::vector<const uint64_t*> ll(wdt * nsub), al(2 * nsub);
+      for (uint32_t i = 0; i < wdt * nsub; i++) ll[i] = k.w[voff + i];
+      for (uint32_t i = 0; i < 2 * nsub; i++) al[i] = k.s2[a_off + i];
+      const uint64_t lb[2] = {lookup_beta.c0, lookup_beta.c1}, lg[2] = {lookup_gamma.c0, lookup_gamma.c1};
+      BJ_TRY(bj_quotient_lookup_specialized(ctx, ll.data(), nsub, wdt, k.consts[c.lookup_table_id_column], k.tables.data(), T,
+                                            k.m, al.data(), k.s2[a_off + 2 * nsub], k.s2[a_off + 2 * nsub + 1], lb, lg,
+                                            powers.data(), n_points, o0, o1));
+    }
+    if (n_gate_terms)
+      BJ_TRY(bj_quotient_gates_general_purpose(ctx, setup->gates.data(), (uint32_t)setup->gates.size(), k.w.data(), V, nullptr, 0,
+                                               k.consts.data(), C, powers.data() + 2 * (size_t)n_lk_terms, n_gate_terms, n_points, o0, o1));
+    {
+      std::vector<uint64_t> nr(V);
+      BJ_TRY(bj_non_residues_for_copy_permutation(n, V, nr.data()));
+      const uint64_t b[2] = {beta.c0, beta.c1}, g[2] = {gamma.c0, gamma.c1};
+      if (split)
+        BJ_TRY(bj_quotient_copy_permutation_with_z_next(ctx, k.w.data(), k.sigma.data(), V, nr.data(), k.s2[0], k.s2[1], (const uint64_t*)z_next.p,
+                                                        (const uint64_t*)z_next.p + nD, n_partial ? k.s2.data() + 2 : nullptr, b, g,
+                                                        powers.data() + 2 * (size_t)(n_lk_terms + n_gate_terms), log_n, log_d, log_q, Q, o0, o1));
+      else
+        BJ_TRY(bj_quotient_copy_permutation(ctx, k.w.data(), k.sigma.data(), V, nr.data(), k.s2[0], k.s2[1],
+                                            n_partial ? k.s2.data() + 2 : nullptr, b, g, powers.data() + 2 * (size_t)(n_lk_terms + n_gate_terms),
+                                            log_n, log_d, log_q, Q, o0, o1));
+    }
+    return bj_quotient_divide_by_vanishing(ctx, o0, o1, log_n, log_q);
+  };
+  if (!streamed) {
+    if (nQl) BJ_TRY(quotient_terms({w_cols, sigma_cols, const_cols, table_cols, s2_cols, m_col}, nQl, q0, q1));
+  } else {
+    // one quotient coset j at a time, under the window of coset j: cosets [0, L) from the kept columns, cosets [L, Q) evaluated
+    // into one coset-sized scratch from the natural-order columns
+    DevMem ev;
+    BJ_TRY(ev.alloc(ctx, (size_t)(2 * V + C + T + (lk ? 1 : 0) + n_s2) * n));
+    for (uint32_t j = 0; j < Q; j++) {
+      QuotientCols k;
+      uint64_t* e = (uint64_t*)ev.p;
+      // columns `kept` moved to coset j, or `cnt` natural columns of `nat` evaluated on coset j into the next slots of ev
+      auto coset_j = [&](const std::vector<const uint64_t*>& kept_cols, const uint64_t* nat, uint32_t cnt, std::vector<const uint64_t*>& out) -> int32_t {
+        out.resize(cnt);
+        if (j < L) {
+          for (uint32_t i = 0; i < cnt; i++) out[i] = kept_cols[i] + (size_t)j * n;
+          return BJ_OK;
+        }
+        if (cnt) BJ_TRY(bj_lde_cosets(ctx, nat, n, e, log_n, log_d, j, j + 1, cnt, 0));
+        for (uint32_t i = 0; i < cnt; i++) out[i] = e + (size_t)i * n;
+        e += (size_t)cnt * n;
+        return BJ_OK;
+      };
+      BJ_TRY(coset_j(w_cols, d_variables, V, k.w));
+      BJ_TRY(coset_j(sigma_cols, setup->sigmas, V, k.sigma));
+      BJ_TRY(coset_j(const_cols, setup->constants, C, k.consts));
+      BJ_TRY(coset_j(table_cols, setup->tables, T, k.tables));
+      BJ_TRY(coset_j(s2_cols, (const uint64_t*)st2.p, n_s2, k.s2));
+      std::vector<const uint64_t*> mj;
+      if (lk) BJ_TRY(coset_j({m_col}, d_multiplicities, 1, mj));
+      k.m = lk ? mj[0] : nullptr;
+      ShardWindow window(ctx, log_q, j);
+      BJ_TRY(quotient_terms(k, n, q0 + (size_t)j * n, q1 + (size_t)j * n));
+    }
   }
-  if (n_gate_terms)
-    BJ_TRY(bj_quotient_gates_general_purpose(ctx, setup->gates.data(), (uint32_t)setup->gates.size(), w_cols.data(), V, nullptr, 0,
-                                             const_cols.data(), C, powers.data() + 2 * (size_t)n_lk_terms, n_gate_terms, nQl, q0, q1));
-  {
-    std::vector<uint64_t> nr(V);
-    BJ_TRY(bj_non_residues_for_copy_permutation(n, V, nr.data()));
-    const uint64_t b[2] = {beta.c0, beta.c1}, g[2] = {gamma.c0, gamma.c1};
-    if (split)
-      BJ_TRY(bj_quotient_copy_permutation_with_z_next(ctx, w_cols.data(), sigma_cols.data(), V, nr.data(), s2_cols[0], s2_cols[1], (const uint64_t*)z_next.p,
-                                                      (const uint64_t*)z_next.p + nD, n_partial ? s2_cols.data() + 2 : nullptr, b, g,
-                                                      powers.data() + 2 * (size_t)(n_lk_terms + n_gate_terms), log_n, log_d, log_q, Q, q0, q1));
-    else
-      BJ_TRY(bj_quotient_copy_permutation(ctx, w_cols.data(), sigma_cols.data(), V, nr.data(), s2_cols[0], s2_cols[1],
-                                          n_partial ? s2_cols.data() + 2 : nullptr, b, g, powers.data() + 2 * (size_t)(n_lk_terms + n_gate_terms),
-                                          log_n, log_d, log_q, Q, q0, q1));
-  }
-  BJ_TRY(bj_quotient_divide_by_vanishing(ctx, q0, q1, log_n, log_q));
-  }  // nQl
   z_next.release();
   if (world > 1) {
     // the one bulk exchange: the quotient cosets recombine (they are interpolated together at size n * Q).  Every rank sends
@@ -1364,20 +1445,38 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   return BJ_OK;
 }
 
-int32_t bj_proof_memory_plan(const bj_circuit* circuit, uint32_t world, uint64_t out[2]) {
-  if (!circuit || !out || world == 0 || (world & (world - 1)) || circuit->log_n == 0 || circuit->log_n > 28 || !is_pow2(circuit->fri_lde_factor) ||
+static int32_t memory_plan_shape(const bj_circuit* circuit, uint32_t world, ProofShape* sh) {
+  if (!circuit || world == 0 || (world & (world - 1)) || circuit->log_n == 0 || circuit->log_n > 28 || !is_pow2(circuit->fri_lde_factor) ||
       circuit->fri_lde_factor < 2 || !is_pow2(circuit->quotient_degree) || !is_pow2(circuit->merkle_tree_cap_size) ||
       circuit->merkle_tree_cap_size < world || circuit->num_variables == 0)
     return BJ_ERR_INVALID_ARG;
+  BJ_TRY(proof_shape(*circuit, world, sh));
+  return sh->sched_len == 0 ? BJ_ERR_INVALID_ARG : BJ_OK;
+}
+
+int32_t bj_proof_memory_plan(const bj_circuit* circuit, uint32_t world, uint64_t out[2]) {
   ProofShape sh;
-  BJ_TRY(proof_shape(*circuit, world, &sh));
-  if (sh.sched_len == 0) return BJ_ERR_INVALID_ARG;
-  out[0] = plan_bytes(sh, false);
-  out[1] = compact_applies(sh) ? plan_bytes(sh, true) : 0;
+  if (!out) return BJ_ERR_INVALID_ARG;
+  BJ_TRY(memory_plan_shape(circuit, world, &sh));
+  out[0] = plan_bytes(sh, PLAN_RESIDENT);
+  out[1] = compact_applies(sh) ? plan_bytes(sh, PLAN_COMPACT) : 0;
+  return BJ_OK;
+}
+
+int32_t bj_proof_memory_plan_streamed(const bj_circuit* circuit, uint32_t world, uint64_t* out) {
+  ProofShape sh;
+  if (!out) return BJ_ERR_INVALID_ARG;
+  BJ_TRY(memory_plan_shape(circuit, world, &sh));
+  *out = streamed_applies(sh) ? plan_bytes(sh, PLAN_STREAMED) : 0;
   return BJ_OK;
 }
 
 int32_t bj_setup_is_compact(const bj_setup* s) { return s ? (s->compact ? 1 : 0) : BJ_ERR_INVALID_ARG; }
+
+int32_t bj_setup_plan(const bj_setup* s) {
+  if (!s) return BJ_ERR_INVALID_ARG;
+  return s->compact ? BJ_PLAN_COMPACT : s->streamed ? BJ_PLAN_STREAMED : BJ_PLAN_RESIDENT;
+}
 
 int32_t bj_setup_memory_plan(const bj_setup* s, uint64_t out[3]) {
   if (!s || !out) return BJ_ERR_INVALID_ARG;

@@ -126,7 +126,9 @@ SIGNATURES = {
     "bj_setup_create": (_i32, [_vp, _vp, _vp, _vp, _vp, _pp]),
     "bj_setup_free": (None, [_vp]),
     "bj_proof_memory_plan": (_i32, [_vp, _u32, _vp]),
+    "bj_proof_memory_plan_streamed": (_i32, [_vp, _u32, _vp]),
     "bj_setup_is_compact": (_i32, [_vp]),
+    "bj_setup_plan": (_i32, [_vp]),
     "bj_setup_memory_plan": (_i32, [_vp, _vp]),
     "bj_setup_get_cap": (_i32, [_vp, _vp]),
     "bj_prove": (_i32, [_vp, _vp, _vp, _vp, _pp]),
@@ -175,6 +177,7 @@ class GateDesc(ctypes.Structure):
                 ("variables_initial_offset", ctypes.c_uint32), ("witnesses_initial_offset", ctypes.c_uint32)]
 
 
+PLAN_RESIDENT, PLAN_COMPACT, PLAN_STREAMED = range(3)  # BJ_PLAN_*
 IDX_VARIABLE, IDX_WITNESS, IDX_CONSTANT_POLY, IDX_TEMPORARY, IDX_CONSTANT_VALUE, IDX_CONSTANT_POLY_SHARED = range(6)
 REL_ADD, REL_DOUBLE, REL_SUB, REL_NEGATE, REL_MUL, REL_SQUARE, REL_INVERSE = range(7)
 

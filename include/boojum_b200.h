@@ -78,10 +78,11 @@ BJ_API const char* bj_last_error(const bj_ctx* ctx);
 /* number of kernels this library launched through ctx so far (for launch accounting) */
 BJ_API uint64_t bj_launch_count(const bj_ctx* ctx);
 /* Device-memory limit of the prover driver on this context (bytes; 0, the default: what the device has free when
- * bj_setup_create runs, plus what the context's pool holds without using it).  bj_setup_create compares the two memory plans
- * of bj_proof_memory_plan with it: RESIDENT if that fits, else COMPACT (one GPU, quotient degree < LDE factor), else
- * BJ_ERR_OOM with both byte counts in the message and no kernel launched.  bj_prove follows the setup's plan and refuses the
- * same way if the limit was lowered below it since. */
+ * bj_setup_create runs, plus what the context's pool holds without using it).  bj_setup_create compares the memory plans of
+ * bj_proof_memory_plan and bj_proof_memory_plan_streamed with it: RESIDENT if that fits, else COMPACT (one GPU, quotient
+ * degree < LDE factor), else STREAMED (one GPU, quotient degree > LDE factor), else BJ_ERR_OOM with every applicable byte
+ * count in the message and no kernel launched.  With quotient degree = LDE factor only RESIDENT applies.  bj_prove follows
+ * the setup's plan and refuses the same way if the limit was lowered below it since. */
 BJ_API int32_t bj_ctx_set_memory_limit(bj_ctx* ctx, uint64_t bytes);
 /* highest device memory the context's pool has had in use (cudaMemPoolAttrUsedMemHigh); reset != 0 restarts the mark.
  * Synchronises.  Memory the library keeps outside the pool (twiddles, coset-power tables, scratch) is not included. */
@@ -494,11 +495,23 @@ BJ_API void bj_setup_free(bj_setup* setup);
  * query answers.  Both are the context pool's allocations replayed in the driver's order plus an upper bound of what the
  * library keeps outside the pool (twiddles, coset-power tables, NTT scratch). */
 BJ_API int32_t bj_proof_memory_plan(const bj_circuit* circuit, uint32_t world, uint64_t out[2]);
-/* 1 if bj_setup_create chose the compact plan, 0 if resident */
+/* The STREAMED plan's bytes, counted the same way (0 when it does not apply: world > 1 or quotient degree <= LDE factor).  With
+ * Q > L the resident plan evaluates every setup, witness and stage-2 column on all Q cosets, and cosets [L, Q) are read by the
+ * quotient only.  The streamed plan evaluates those columns on the committed cosets [0, L) only (stride n * L) and keeps the
+ * natural-order stage-2 columns.  The quotient then runs one coset j at a time: coset j < L from the kept columns, coset
+ * j >= L evaluated from the natural-order columns into one coset-sized scratch of every column the quotient reads.  Proofs
+ * are bit-identical to the resident plan's. */
+BJ_API int32_t bj_proof_memory_plan_streamed(const bj_circuit* circuit, uint32_t world, uint64_t* out);
+/* 1 if bj_setup_create chose the compact plan, 0 otherwise (resident or streamed) */
 BJ_API int32_t bj_setup_is_compact(const bj_setup* setup);
+/* the plan bj_setup_create chose: BJ_PLAN_RESIDENT, BJ_PLAN_COMPACT or BJ_PLAN_STREAMED */
+#define BJ_PLAN_RESIDENT 0
+#define BJ_PLAN_COMPACT 1
+#define BJ_PLAN_STREAMED 2
+BJ_API int32_t bj_setup_plan(const bj_setup* setup);
 /* the plan bj_setup_create chose: out[0] the peak bytes of the context's pool over bj_setup_create + bj_prove (what
  * bj_ctx_memory_high_water reads on a fresh context), out[1] the bound on what the library holds outside the pool, out[2] the
- * columns the compact plan recomputes at a time (0 on the resident plan) */
+ * columns the compact plan recomputes at a time (0 on the resident and streamed plans) */
 BJ_API int32_t bj_setup_memory_plan(const bj_setup* setup, uint64_t out[3]);
 BJ_API int32_t bj_setup_get_cap(const bj_setup* setup, uint64_t* h_cap /* 4 * cap_size u64: VerificationKey::setup_merkle_tree_cap */);
 BJ_API int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables, const uint64_t* d_multiplicities /* or NULL */,
