@@ -474,3 +474,207 @@ API void orc_deep_group(uint64_t *acc0, uint64_t *acc1, const uint64_t *const *s
     acc1[t] = gl_add(gl_canon(acc1[t]), s.c1);
   }
 }
+
+/* ------------------------------------------------------------------------------------------------
+ * Copy-permutation argument (stage 2 and its quotient terms)
+ * Fp2 values are (c0, c1) column pairs; k_j are the non-residues of make_non_residues
+ * (src/cs/implementations/utils.rs:636-688), passed in by the caller.
+ * ---------------------------------------------------------------------------------------------- */
+static inline gl2_t gl2_of(const uint64_t *c0, const uint64_t *c1, size_t i) {
+  return (gl2_t){gl_canon(c0[i]), gl_canon(c1[i])};
+}
+static inline gl2_t gl2_canon2(const uint64_t v[2]) { return (gl2_t){gl_canon(v[0]), gl_canon(v[1])}; }
+
+/* w + beta * s + gamma for base-field w and s */
+static inline gl2_t cp_factor(uint64_t w, uint64_t s, gl2_t beta, gl2_t gamma) {
+  return gl2_add(gl2_add(gl2_mul_base(beta, gl_canon(s)), (gl2_t){gl_canon(w), 0}), gamma);
+}
+
+/* R_c(x_i) = prod_{j in chunk c} (w_j + beta k_j x_i + gamma) / (w_j + beta sigma_j + gamma),  x_i = omega_n^i
+ *                                                      pointwise_rational_in_extension, copy_permutation.rs:114-248 */
+static gl2_t cp_ratio(const uint64_t *const *vars, const uint64_t *const *sigmas, const uint64_t *ks, size_t c0, size_t c1,
+                      size_t i, uint64_t x, gl2_t beta, gl2_t gamma) {
+  gl2_t num = {1, 0}, den = {1, 0};
+  for (size_t j = c0; j < c1; j++) {
+    num = gl2_mul(num, cp_factor(vars[j][i], gl_mul(gl_canon(ks[j]), x), beta, gamma));
+    den = gl2_mul(den, cp_factor(vars[j][i], sigmas[j][i], beta, gamma));
+  }
+  return gl2_mul(num, gl2_inv(den));
+}
+
+/* compute_partial_products_in_extension                 src/cs/implementations/copy_permutation.rs:649-766
+ * z[i] = prod_{t < i} prod_c R_c[t] (shifted_grand_product_in_extension, :425-510), p_c = z * R_0 * ... * R_c for every
+ * chunk but the last.  Chunks are `chunk` consecutive columns.  partials: [n_chunks - 1][2][n] (may be NULL for one chunk).
+ * grand[2] receives prod over all rows of prod_c R_c (one for a satisfied copy permutation). */
+API void orc_cp_stage2(const uint64_t *const *vars, const uint64_t *const *sigmas, size_t n_cols, const uint64_t *ks,
+                       const uint64_t beta_in[2], const uint64_t gamma_in[2], unsigned log_n, size_t chunk, uint64_t *z0,
+                       uint64_t *z1, uint64_t *partials, uint64_t grand[2]) {
+  size_t n = (size_t)1 << log_n, n_chunks = (n_cols + chunk - 1) / chunk;
+  gl2_t beta = gl2_canon2(beta_in), gamma = gl2_canon2(gamma_in);
+  uint64_t w = gl_omega(log_n);
+  /* almost_z[i] = prod_c R_c[i], into z */
+#pragma omp parallel for schedule(static)
+  for (long i = 0; i < (long)n; i++) {
+    uint64_t x = gl_pow(w, (uint64_t)i);
+    gl2_t az = {1, 0};
+    for (size_t c = 0; c < n_chunks; c++) {
+      size_t e = (c + 1) * chunk < n_cols ? (c + 1) * chunk : n_cols;
+      az = gl2_mul(az, cp_ratio(vars, sigmas, ks, c * chunk, e, (size_t)i, x, beta, gamma));
+    }
+    z0[i] = az.c0;
+    z1[i] = az.c1;
+  }
+  /* exclusive prefix product, serially */
+  gl2_t run = {1, 0};
+  for (size_t i = 0; i < n; i++) {
+    gl2_t a = {z0[i], z1[i]};
+    z0[i] = run.c0;
+    z1[i] = run.c1;
+    run = gl2_mul(run, a);
+  }
+  grand[0] = run.c0;
+  grand[1] = run.c1;
+  if (n_chunks < 2) return;
+#pragma omp parallel for schedule(static)
+  for (long i = 0; i < (long)n; i++) {
+    uint64_t x = gl_pow(w, (uint64_t)i);
+    gl2_t p = {z0[i], z1[i]};
+    for (size_t c = 0; c + 1 < n_chunks; c++) {
+      p = gl2_mul(p, cp_ratio(vars, sigmas, ks, c * chunk, (c + 1) * chunk, (size_t)i, x, beta, gamma));
+      partials[(2 * c) * n + (size_t)i] = p.c0;
+      partials[(2 * c + 1) * n + (size_t)i] = p.c1;
+    }
+  }
+}
+
+/* x(t) = 7 * omega_{2^bits}^{bitrev_bits(t)}: the point of flat LDE index t (coset-major, bit-reversed inside a coset) */
+static inline uint64_t lde_point(size_t t, unsigned bits) { return gl_mul(GL_MULT_GEN, gl_pow(gl_omega(bits), gl_bitrev(t, bits))); }
+
+/* Quotient terms of the copy permutation at the flat LDE indices t < 2^(log_n + log_q), ADDED to q:
+ *   alpha_0 (z - 1) (x^n - 1) / (x - 1)                                 prover.rs:1189-1227 (z(1) = 1)
+ *   alpha_{c+1} (lhs_c prod_j (w_j + beta sigma_j + gamma) - rhs_c prod_j (w_j + beta k_j x + gamma))
+ *     lhs = p_0, ..., p_{m-2}, z(omega x);  rhs = z, p_0, ..., p_{m-2}    copy_permutation.rs:1000-1249
+ *   z(omega x) at bitrev(bitrev(i) + 1) of the same coset                utils.rs:1245-1271
+ * var_ldes, sigma_ldes, z, partials (c0, c1 of each, 2 * (n_chunks - 1) pointers): flat LDEs of factor 2^log_lde. */
+API void orc_cp_quotient(const uint64_t *const *var_ldes, const uint64_t *const *sigma_ldes, size_t n_cols, const uint64_t *ks,
+                         const uint64_t *z0, const uint64_t *z1, const uint64_t *const *partials, const uint64_t beta_in[2],
+                         const uint64_t gamma_in[2], const uint64_t *alphas, unsigned log_n, unsigned log_lde, unsigned log_q,
+                         size_t chunk, uint64_t *q0, uint64_t *q1) {
+  size_t n = (size_t)1 << log_n, n_chunks = (n_cols + chunk - 1) / chunk;
+  size_t n_points = n << log_q;
+  gl2_t beta = gl2_canon2(beta_in), gamma = gl2_canon2(gamma_in);
+#pragma omp parallel for schedule(static)
+  for (long tl = 0; tl < (long)n_points; tl++) {
+    size_t t = (size_t)tl, coset = t >> log_n, i = t & (n - 1);
+    uint64_t x = lde_point(t, log_n + log_lde);
+    size_t tsh = (coset << log_n) | gl_bitrev((gl_bitrev(i, log_n) + 1) & (n - 1), log_n);
+    gl2_t z = gl2_of(z0, z1, t);
+    uint64_t l1 = gl_mul(gl_sub(gl_pow(x, n), 1), gl_inv(gl_sub(x, 1)));
+    gl2_t q = gl2_mul(gl2_mul_base(gl2_sub(z, (gl2_t){1, 0}), l1), gl2_canon2(alphas));
+    for (size_t c = 0; c < n_chunks; c++) {
+      gl2_t lhs = c + 1 < n_chunks ? gl2_of(partials[2 * c], partials[2 * c + 1], t) : gl2_of(z0, z1, tsh);
+      gl2_t rhs = c == 0 ? z : gl2_of(partials[2 * (c - 1)], partials[2 * (c - 1) + 1], t);
+      size_t e = (c + 1) * chunk < n_cols ? (c + 1) * chunk : n_cols;
+      for (size_t j = c * chunk; j < e; j++) {
+        lhs = gl2_mul(lhs, cp_factor(var_ldes[j][t], sigma_ldes[j][t], beta, gamma));
+        rhs = gl2_mul(rhs, cp_factor(var_ldes[j][t], gl_mul(gl_canon(ks[j]), x), beta, gamma));
+      }
+      q = gl2_add(q, gl2_mul(gl2_sub(lhs, rhs), gl2_canon2(alphas + 2 * (c + 1))));
+    }
+    q0[t] = gl_add(gl_canon(q0[t]), q.c0);
+    q1[t] = gl_add(gl_canon(q1[t]), q.c1);
+  }
+}
+
+/* divide_by_vanishing_for_bitreversed_coset_enumeration      utils.rs:770-817
+ * q[t] /= x^n - 1 on the first 2^log_q cosets of the size-n*2^log_q domain (one constant per coset) */
+API void orc_divide_by_vanishing(uint64_t *q0, uint64_t *q1, unsigned log_n, unsigned log_q) {
+  size_t n = (size_t)1 << log_n, Q = (size_t)1 << log_q;
+  for (size_t j = 0; j < Q; j++) {
+    uint64_t shift = gl_mul(GL_MULT_GEN, gl_pow(gl_omega(log_n + log_q), gl_bitrev(j, log_q)));
+    uint64_t m = gl_inv(gl_sub(gl_pow(shift, n), 1));
+#pragma omp parallel for schedule(static)
+    for (long i = 0; i < (long)n; i++) {
+      size_t t = j * n + (size_t)i;
+      q0[t] = gl_mul(gl_canon(q0[t]), m);
+      q1[t] = gl_mul(gl_canon(q1[t]), m);
+    }
+  }
+}
+
+/* ------------------------------------------------------------------------------------------------
+ * Log-derivative lookup argument over specialised columns       src/cs/implementations/lookup_argument_in_ext.rs
+ * A sub-argument's tuple is `width` lookup columns, then the table id column if there is one; the table has
+ * n_table_cols = width (+ 1) columns.  agg(cols) = beta + sum_j gamma^j cols[j].
+ * ---------------------------------------------------------------------------------------------- */
+static gl2_t lookup_agg(const uint64_t *const *cols, size_t n, const uint64_t *extra, size_t r, gl2_t beta, gl2_t gamma) {
+  gl2_t acc = beta, g = {1, 0};
+  for (size_t j = 0; j < n; j++) {
+    acc = gl2_add(acc, gl2_mul_base(g, gl_canon(cols[j][r])));
+    g = gl2_mul(g, gamma);
+  }
+  if (extra) acc = gl2_add(acc, gl2_mul_base(g, gl_canon(extra[r])));
+  return acc;
+}
+
+/* compute_lookup_poly_pairs_specialized                   :320-947
+ * out [n_sub + 1][2][n]: A_i = 1 / agg(tuple_i), then B = m / agg(table) */
+API void orc_lookup_polys(const uint64_t *const *lookup_cols, size_t n_sub, size_t width, const uint64_t *table_id,
+                          const uint64_t *const *table_cols, size_t n_table_cols, const uint64_t *mult, const uint64_t beta_in[2],
+                          const uint64_t gamma_in[2], size_t n, uint64_t *out) {
+  gl2_t beta = gl2_canon2(beta_in), gamma = gl2_canon2(gamma_in);
+#pragma omp parallel for schedule(static)
+  for (long rl = 0; rl < (long)n; rl++) {
+    size_t r = (size_t)rl;
+    for (size_t i = 0; i < n_sub; i++) {
+      gl2_t a = gl2_inv(lookup_agg(lookup_cols + i * width, width, table_id, r, beta, gamma));
+      out[(2 * i) * n + r] = a.c0;
+      out[(2 * i + 1) * n + r] = a.c1;
+    }
+    gl2_t b = gl2_mul_base(gl2_inv(lookup_agg(table_cols, n_table_cols, NULL, r, beta, gamma)), gl_canon(mult[r]));
+    out[(2 * n_sub) * n + r] = b.c0;
+    out[(2 * n_sub + 1) * n + r] = b.c1;
+  }
+}
+
+/* compute_quotient_terms_for_lookup_specialized           :949-1319, ADDED to q at points t < n_points:
+ *   alpha_i (A_i agg(tuple_i) - 1) for each sub-argument, alpha_{n_sub} (B agg(table) - m)
+ * a_ldes: 2 * n_sub pointers (c0, c1 of each A_i) */
+API void orc_lookup_quotient(const uint64_t *const *lookup_ldes, size_t n_sub, size_t width, const uint64_t *table_id,
+                             const uint64_t *const *table_ldes, size_t n_table_cols, const uint64_t *mult,
+                             const uint64_t *const *a_ldes, const uint64_t *b0, const uint64_t *b1, const uint64_t beta_in[2],
+                             const uint64_t gamma_in[2], const uint64_t *alphas, size_t n_points, uint64_t *q0, uint64_t *q1) {
+  gl2_t beta = gl2_canon2(beta_in), gamma = gl2_canon2(gamma_in);
+#pragma omp parallel for schedule(static)
+  for (long tl = 0; tl < (long)n_points; tl++) {
+    size_t t = (size_t)tl;
+    gl2_t q = {0, 0};
+    for (size_t i = 0; i < n_sub; i++) {
+      gl2_t d = lookup_agg(lookup_ldes + i * width, width, table_id, t, beta, gamma);
+      gl2_t v = gl2_sub(gl2_mul(d, gl2_of(a_ldes[2 * i], a_ldes[2 * i + 1], t)), (gl2_t){1, 0});
+      q = gl2_add(q, gl2_mul(v, gl2_canon2(alphas + 2 * i)));
+    }
+    gl2_t d = lookup_agg(table_ldes, n_table_cols, NULL, t, beta, gamma);
+    gl2_t v = gl2_sub(gl2_mul(d, gl2_of(b0, b1, t)), (gl2_t){gl_canon(mult[t]), 0});
+    q = gl2_add(q, gl2_mul(v, gl2_canon2(alphas + 2 * n_sub)));
+    q0[t] = gl_add(gl_canon(q0[t]), q.c0);
+    q1[t] = gl_add(gl_canon(q1[t]), q.c1);
+  }
+}
+
+/* ------------------------------------------------------------------------------------------------
+ * f(at) by Horner for base-field coefficient columns (low degree first) at an Fp2 point: with orc_intt_n2n, the
+ * definition that barycentric_evaluate_*_at_extension (utils.rs:907-1243) computes in another way.
+ * out: [n_cols][2]
+ * ---------------------------------------------------------------------------------------------- */
+API void orc_horner_ext(const uint64_t *mono, size_t n_cols, size_t n, const uint64_t at_in[2], uint64_t *out) {
+  gl2_t at = gl2_canon2(at_in);
+#pragma omp parallel for schedule(static)
+  for (long c = 0; c < (long)n_cols; c++) {
+    const uint64_t *m = mono + (size_t)c * n;
+    gl2_t acc = {0, 0};
+    for (size_t i = n; i-- > 0;) acc = gl2_add(gl2_mul(acc, at), (gl2_t){gl_canon(m[i]), 0});
+    out[2 * c] = acc.c0;
+    out[2 * c + 1] = acc.c1;
+  }
+}

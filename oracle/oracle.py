@@ -17,9 +17,10 @@ MULT_GEN = 7
 
 
 def build(force=False):
-    """Compile oracle/liboracle.so with the system gcc (oracle/Makefile)."""
-    if force or not os.path.exists(_LIB_PATH):
-        subprocess.check_call(["make", "-C", _HERE, "-s"])
+    """Compile oracle/liboracle.so with the system gcc (oracle/Makefile).  make runs every time and rebuilds the library
+    when a source is newer, so a library built from an older oracle.c (one that lacks symbols lib() looks up) is not
+    loaded; an up-to-date library is left alone, so a read-only tree works once it is built."""
+    subprocess.check_call(["make", "-C", _HERE, "-s"] + (["-B"] if force else []))
     return _LIB_PATH
 
 
@@ -55,6 +56,13 @@ def lib():
             "orc_batch_inverse_ext": (None, [vp, vp, sz]),
             "orc_deep_point": (None, [vp, vp, vp, vp, vp, vp, vp, sz, u64, vp]),
             "orc_deep_group": (None, [vp, vp, vp, vp, sz, vp, vp, vp, ctypes.c_uint]),
+            "orc_cp_stage2": (None, [vp, vp, sz, vp, vp, vp, ctypes.c_uint, sz, vp, vp, vp, vp]),
+            "orc_cp_quotient": (None, [vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, ctypes.c_uint, ctypes.c_uint, ctypes.c_uint, sz,
+                                       vp, vp]),
+            "orc_divide_by_vanishing": (None, [vp, vp, ctypes.c_uint, ctypes.c_uint]),
+            "orc_lookup_polys": (None, [vp, sz, sz, vp, vp, sz, vp, vp, vp, sz, vp]),
+            "orc_lookup_quotient": (None, [vp, sz, sz, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, sz, vp, vp]),
+            "orc_horner_ext": (None, [vp, sz, sz, vp, vp]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)
@@ -285,6 +293,97 @@ def deep_group(acc0, acc1, sources, values_at, challenges, at):
     at_ = _u64(np.array(at, dtype=np.uint64))
     lib().orc_deep_group(_p(a0), _p(a1), p0, p1, n, _p(vals), _p(chs), _p(at_), a0.shape[0].bit_length() - 1)
     return a0, a1
+
+
+# ----------------------------------------------------------- copy permutation / lookup / openings -----
+def _ptrs(cols):
+    """list of 1-D uint64 arrays -> (ctypes pointer array, contiguous arrays kept alive by the caller)"""
+    arrs = [_u64(c).reshape(-1) for c in cols]
+    return (ctypes.c_void_p * max(1, len(arrs)))(*[a.ctypes.data for a in arrs]), arrs
+
+
+def _e2(v):
+    return _u64(np.array([int(v[0]), int(v[1])], dtype=np.uint64))
+
+
+def cp_stage2(variables, sigmas, non_residues, beta, gamma, chunk):
+    """compute_partial_products_in_extension (cs/implementations/copy_permutation.rs:649-766).  variables / sigmas: lists of
+    [n] columns (natural order).  Returns (z_c0, z_c1, partials [n_chunks - 1, 2, n], grand product (c0, c1))."""
+    n_cols, n = len(variables), _u64(variables[0]).shape[0]
+    n_chunks = (n_cols + chunk - 1) // chunk
+    pv, kv = _ptrs(variables)
+    ps, ks_ = _ptrs(sigmas)
+    ks = _u64(non_residues)
+    z0, z1 = np.zeros(n, np.uint64), np.zeros(n, np.uint64)
+    partials = np.zeros((max(n_chunks - 1, 1), 2, n), np.uint64)
+    grand = np.zeros(2, np.uint64)
+    lib().orc_cp_stage2(pv, ps, n_cols, _p(ks), _p(_e2(beta)), _p(_e2(gamma)), n.bit_length() - 1, chunk, _p(z0), _p(z1),
+                        _p(partials), _p(grand))
+    return z0, z1, partials[:n_chunks - 1], (int(grand[0]), int(grand[1]))
+
+
+def cp_quotient(var_ldes, sigma_ldes, non_residues, z, partials, beta, gamma, alphas, log_n, log_lde, log_q, chunk, q0, q1):
+    """copy-permutation quotient terms and the z(1) = 1 term (copy_permutation.rs:1000-1249, prover.rs:1189-1227) on the
+    first 2^log_q cosets, added to (q0, q1).  *_ldes, z, partials: flat [L * n] LDE columns; partials: list of (c0, c1)."""
+    pv, kv = _ptrs(var_ldes)
+    ps, ks_ = _ptrs(sigma_ldes)
+    pp, kp = _ptrs([t for pr in partials for t in pr])
+    z0, z1 = _u64(z[0]).reshape(-1), _u64(z[1]).reshape(-1)
+    al = _u64(np.array(alphas, dtype=np.uint64).reshape(-1))
+    ks = _u64(non_residues)
+    o0, o1 = _u64(q0).copy(), _u64(q1).copy()
+    lib().orc_cp_quotient(pv, ps, len(var_ldes), _p(ks), _p(z0), _p(z1), pp, _p(_e2(beta)), _p(_e2(gamma)), _p(al), log_n,
+                          log_lde, log_q, chunk, _p(o0), _p(o1))
+    return o0, o1
+
+
+def divide_by_vanishing(q0, q1, log_n, log_q):
+    """divide_by_vanishing_for_bitreversed_coset_enumeration (cs/implementations/utils.rs:770-817)."""
+    o0, o1 = _u64(q0).copy(), _u64(q1).copy()
+    assert o0.shape[0] == 1 << (log_n + log_q)
+    lib().orc_divide_by_vanishing(_p(o0), _p(o1), log_n, log_q)
+    return o0, o1
+
+
+def lookup_polys(lookup_cols, width, table_id_col, table_cols, multiplicity, beta, gamma):
+    """compute_lookup_poly_pairs_specialized (cs/implementations/lookup_argument_in_ext.rs:320-947).  lookup_cols: n_sub * width
+    columns.  Returns [n_sub + 1, 2, n]: A_0 .. A_{n_sub - 1}, then B."""
+    n_sub = len(lookup_cols) // width
+    pl, kl = _ptrs(lookup_cols)
+    pt, kt = _ptrs(table_cols)
+    tid = _u64(table_id_col) if table_id_col is not None else None
+    m = _u64(multiplicity)
+    n = m.shape[0]
+    out = np.zeros((n_sub + 1, 2, n), np.uint64)
+    lib().orc_lookup_polys(pl, n_sub, width, _p(tid) if tid is not None else None, pt, len(table_cols), _p(m), _p(_e2(beta)),
+                           _p(_e2(gamma)), n, _p(out))
+    return out
+
+
+def lookup_quotient(lookup_ldes, width, table_id_lde, table_ldes, multiplicity_lde, a_ldes, b_lde, beta, gamma, alphas, q0, q1):
+    """compute_quotient_terms_for_lookup_specialized (lookup_argument_in_ext.rs:949-1319) at the points of (q0, q1), added to
+    them.  a_ldes: list of (c0, c1); b_lde: (c0, c1)."""
+    n_sub = len(lookup_ldes) // width
+    pl, kl = _ptrs(lookup_ldes)
+    pt, kt = _ptrs(table_ldes)
+    pa, ka = _ptrs([t for pr in a_ldes for t in pr])
+    tid = _u64(table_id_lde).reshape(-1) if table_id_lde is not None else None
+    m, b0, b1 = _u64(multiplicity_lde).reshape(-1), _u64(b_lde[0]).reshape(-1), _u64(b_lde[1]).reshape(-1)
+    al = _u64(np.array(alphas, dtype=np.uint64).reshape(-1))
+    o0, o1 = _u64(q0).copy(), _u64(q1).copy()
+    lib().orc_lookup_quotient(pl, n_sub, width, _p(tid) if tid is not None else None, pt, len(table_ldes), _p(m), pa, _p(b0),
+                              _p(b1), _p(_e2(beta)), _p(_e2(gamma)), _p(al), o0.shape[0], _p(o0), _p(o1))
+    return o0, o1
+
+
+def horner_ext(monomials, at):
+    """f(at) for each row of [n_cols, n] base-field coefficients (low degree first) at an Fp2 point -> [n_cols, 2]."""
+    m = _u64(monomials)
+    if m.ndim == 1:
+        m = m[None, :]
+    out = np.zeros((m.shape[0], 2), np.uint64)
+    lib().orc_horner_ext(_p(m), m.shape[0], m.shape[1], _p(_e2(at)), _p(out))
+    return out
 
 
 def random_field(rng, shape):
