@@ -242,9 +242,9 @@ class Context:
 
     def set_memory_limit(self, nbytes):
         """bj_ctx_set_memory_limit: device bytes a proof on this context may use (0: what is free when the setup is created).
-        native_setup picks the resident plan if it fits, else the compact one (quotient degree < LDE factor), else the streamed
-        one (quotient degree > LDE factor), and raises BoojumError (out of device memory, with every applicable plan's byte
-        count) if none does."""
+        native_setup picks the resident plan if it fits, else the compact one (quotient degree < LDE factor, one GPU), else the
+        streamed one (quotient degree > LDE factor, one GPU or a sharded context), and raises BoojumError (out of device
+        memory, with every applicable plan's byte count) if none does."""
         self._check(lib.bj_ctx_set_memory_limit(self._h, int(nbytes)))
 
     def memory_high_water(self, reset=False):
@@ -680,9 +680,10 @@ class Comm:
 
 def proof_memory_plan(log_n, num_variables, num_constants, quotient_degree, config, lookup=None, world=1):
     """bj_proof_memory_plan: device bytes of native_setup + prove at their peak on each of `world` GPUs, counted from the
-    shapes (no device needed).  -> dict(resident=bytes, compact=bytes or None, streamed=bytes or None), None where the plan
-    does not apply (compact: one GPU with quotient degree < LDE factor; streamed: one GPU with quotient degree > LDE factor,
-    bj_proof_memory_plan_streamed)."""
+    shapes (no device needed).  -> dict(resident=bytes, compact=bytes or None, streamed=bytes or None,
+    streamed_sharded=bytes or None), None where the plan does not apply (compact: one GPU with quotient degree < LDE factor;
+    streamed: one GPU with quotient degree > LDE factor, bj_proof_memory_plan_streamed; streamed_sharded: the streamed plan on
+    each of `world` GPUs, quotient degree > LDE factor, bj_proof_memory_plan_streamed_sharded)."""
     c = native.Circuit()
     c.log_n, c.num_variables, c.num_constants, c.quotient_degree = log_n, num_variables, num_constants, quotient_degree
     c.fri_lde_factor, c.merkle_tree_cap_size = config.fri_lde_factor, config.merkle_tree_cap_size
@@ -693,7 +694,10 @@ def proof_memory_plan(log_n, num_variables, num_constants, quotient_degree, conf
     _ok(lib.bj_proof_memory_plan(ctypes.byref(c), world, out), "bj_proof_memory_plan")
     streamed = ctypes.c_uint64()
     _ok(lib.bj_proof_memory_plan_streamed(ctypes.byref(c), world, ctypes.byref(streamed)), "bj_proof_memory_plan_streamed")
-    return {"resident": int(out[0]), "compact": int(out[1]) or None, "streamed": int(streamed.value) or None}
+    sharded = ctypes.c_uint64()
+    _ok(lib.bj_proof_memory_plan_streamed_sharded(ctypes.byref(c), world, ctypes.byref(sharded)), "bj_proof_memory_plan_streamed_sharded")
+    return {"resident": int(out[0]), "compact": int(out[1]) or None, "streamed": int(streamed.value) or None,
+            "streamed_sharded": int(sharded.value) or None}
 
 
 def _circuit(ctx, log_n, num_variables, num_constants, gates, lookup):

@@ -75,11 +75,14 @@ struct CosetShard {
   }
   // the window of one coset j of 2^log_cosets: a buffer that holds coset j alone is the local layout of rank j in a coset
   // shard of world 2^log_cosets, so the row-local kernels reading it get global_index(t) = j * n + t, the coset's x(t) and
-  // vanishing constant, and z(omega x) inside the same coset, exactly as on the whole domain
-  __host__ static CosetShard window(uint32_t log_cosets, uint32_t j) {
+  // vanishing constant, and z(omega x) inside the same coset, exactly as on the whole domain.  With log_split > 0 the window
+  // is of one unit u of 2^log_units (a row block of a coset): the layout of rank u in a split shard of world 2^log_units, so
+  // bj_lde evaluates that unit alone (the split shard's fold + row-block transform) and the kernels see its global indices.
+  __host__ static CosetShard window(uint32_t log_units, uint32_t u, uint32_t log_split = 0) {
     CosetShard w;
-    w.first = j;
-    w.log_stride = log_cosets;
+    w.first = u;
+    w.log_stride = log_units;
+    w.log_split = log_split;
     return w;
   }
 };

@@ -181,19 +181,12 @@ static int32_t keep_first_cosets_grouped(bj_ctx* ctx, ColumnGroups& g, std::vect
   return BJ_OK;
 }
 
-// the LDE columns a plan keeps: every coset of the factor-2^log_d domain (lde_columns), or on the streamed plan only the
-// first `streamed_cosets` = L, stride n * L (bj_lde_cosets: the same coset transforms, so the values are bit-identical)
-static int32_t lde_kept(bj_ctx* ctx, const uint64_t* d_in, uint64_t* d_out, u32 log_n, u32 log_d, u32 n_cols, u32 streamed_cosets) {
-  if (!streamed_cosets) return lde_columns(ctx, d_in, d_out, log_n, log_d, n_cols);
-  return n_cols ? bj_lde_cosets(ctx, d_in, 1ull << log_n, d_out, log_n, log_d, 0, streamed_cosets, n_cols, 0) : BJ_OK;
-}
-
-// streamed plan: while the quotient kernels of coset j run on a buffer that holds coset j alone, the context's shard is
-// the window of coset j; the caller's shard comes back on every exit path
+// streamed plan: while the quotient kernels of unit u run on a buffer that holds unit u alone, the context's shard is
+// the window of unit u; the caller's shard comes back on every exit path
 struct ShardWindow {
   bj_ctx* ctx;
   CosetShard saved;
-  ShardWindow(bj_ctx* c, u32 log_cosets, u32 j) : ctx(c), saved(c->shard) { c->shard = CosetShard::window(log_cosets, j); }
+  ShardWindow(bj_ctx* c, u32 log_units, u32 u, u32 log_split) : ctx(c), saved(c->shard) { c->shard = CosetShard::window(log_units, u, log_split); }
   ~ShardWindow() { ctx->shard = saved; }
   ShardWindow(const ShardWindow&) = delete;
   ShardWindow& operator=(const ShardWindow&) = delete;
@@ -267,9 +260,11 @@ struct QueryAnswer {
 // keeps only the first Q cosets of the setup, witness and stage-2 columns once their trees are built: the quotient reads
 // cosets [0, Q) and the openings coset 0, so cosets [Q, L) are read by DEEP and the query answers only, and those two
 // recompute them from the natural-order columns, a chunk of columns and one coset at a time.  The quotient oracle stays
-// resident.  STREAMED (one GPU, Q > L) evaluates the setup, witness and stage-2 columns on the committed cosets [0, L) only:
+// resident.  STREAMED (Q > L) evaluates the setup, witness and stage-2 columns on the committed cosets [0, L) only:
 // cosets [L, Q) are read by the quotient alone, which evaluates every column it reads onto one such coset at a time into a
-// coset-sized scratch, from the natural-order columns (the stage-2 ones are kept for it).  The plan replays the driver's
+// coset-sized scratch, from the natural-order columns (the stage-2 ones are kept for it).  On a sharded context each rank
+// keeps its units of the committed cosets and evaluates its own units of cosets [L, Q), one unit (a coset, or a row block
+// of one on a split shard, with its z(omega x) columns) at a time into a unit-sized scratch.  The plan replays the driver's
 // stream-ordered pool allocations in order (pool_peak) and adds what the library keeps outside the pool (library_reserve):
 // twiddles, coset-power tables and the NTT scratch.
 enum MemoryPlan : u32 { PLAN_RESIDENT = BJ_PLAN_RESIDENT, PLAN_COMPACT = BJ_PLAN_COMPACT, PLAN_STREAMED = BJ_PLAN_STREAMED };
@@ -376,7 +371,7 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk) {
     m.add(s.n_s2 * nD);
     lde_groups(s.n_s2);
   }
-  const u64 zn = s.split ? 2 * nD : 0;
+  const u64 zn = s.split && !streamed ? 2 * nD : 0;  // the streamed plan evaluates z(omega x) per unit, into its scratch
   if (zn) m.add(zn);
   // the compact plan keeps the natural stage-2 columns for DEEP and the queries, the streamed plan for the quotient
   if (!compact && !streamed) m.sub(s.n_s2 * n);
@@ -388,12 +383,13 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk) {
     }
   // round 3
   m.add(2 * nQ);
-  if (streamed) {  // one coset of every column the quotient reads
-    m.add((u64)s.nat_cols() * n);
-    m.sub((u64)s.nat_cols() * n);
-  }
   const u64 nQl = ((u64)s.Q << s.split) >= w ? nQ / w : n >> s.split;
   if (w > 1) m.add(2 * std::max<u64>(nQl, 1));
+  if (streamed) {  // one unit of every column the quotient reads (and of z(omega x) on a split shard)
+    const u64 unit = (u64)(s.nat_cols() + (s.split ? 2 : 0)) * (n >> s.split);
+    m.add(unit);
+    m.sub(unit);
+  }
   if (zn) m.sub(zn);
   if (w > 1) {
     const u64 per = std::max<u64>(1, ((u64)s.Q << s.split) / w), nb = n >> s.split;
@@ -467,7 +463,7 @@ static u64 library_reserve(const ProofShape& s) {
 }
 
 static bool compact_applies(const ProofShape& s) { return s.world == 1 && s.Q < s.L; }
-static bool streamed_applies(const ProofShape& s) { return s.world == 1 && s.Q > s.L; }
+static bool streamed_applies(const ProofShape& s) { return s.Q > s.L; }  // on one GPU and on sharded contexts
 
 static u64 plan_bytes(const ProofShape& s, MemoryPlan plan, u32 chunk = 2) { return pool_peak(s, plan, chunk) + library_reserve(s); }
 
@@ -483,7 +479,7 @@ struct bj_setup {
   uint32_t n_tables = 0;
   bj::DevMem lde;  // [V + C + T][D][n], D = max(L, quotient degree): the tree commits to the first L cosets of every column
   bj::Oracle tree;
-  uint64_t col_len = 0;  // elements of one LDE column held by this context: n * (D / world), n * Q compact, n * L streamed
+  uint64_t col_len = 0;  // elements of one LDE column held by this context: n * (D / world), n * Q compact, n * (L / world) streamed
   bool compact = false;   // memory plan chosen by bj_setup_create, followed by bj_prove
   bool streamed = false;
   uint64_t limit = 0;    // the device-memory limit the plan was chosen under
@@ -595,8 +591,9 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
   }
   std::unique_ptr<bj_setup> s(new bj_setup());
   {
-    // the memory plan: resident if it fits under the limit, else compact (Q < L), else streamed (Q > L); refused before
-    // anything is launched
+    // the memory plan: resident if it fits under the limit, else compact (Q < L, one GPU), else streamed (Q > L); refused
+    // before anything is launched.  On a sharded context every rank chooses under its own limit: the resident and streamed
+    // plans hold the same committed units and run the same collectives, so ranks on different plans still agree
     ProofShape sh;
     BJ_TRY(proof_shape(*circuit, comm_world(ctx), &sh));
     s->plan[0] = plan_bytes(sh, PLAN_RESIDENT);
@@ -656,14 +653,15 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
   const uint32_t V = circuit->num_variables, C = circuit->num_constants, T = s->n_tables;
   const uint32_t log_n = circuit->log_n, log_l = s->log_l(), log_d = s->log_d();
   const u64 n = 1ull << log_n;
-  // the streamed plan evaluates the committed cosets [0, L) only; the quotient recomputes the others from the borrowed
-  // natural-order columns
-  const uint32_t kept = s->streamed ? circuit->fri_lde_factor : 0;
-  s->col_len = s->streamed ? n << log_l : (n << log_d) / comm_world(ctx);
+  // the streamed plan evaluates the committed cosets [0, L) only (this rank's units of them): the LDE at factor L, whose
+  // cosets are the first L of the factor-D domain with the same shifts, so the values and trees do not change.  The
+  // quotient recomputes the other cosets from the borrowed natural-order columns.
+  const uint32_t log_kept = s->streamed ? log_l : log_d;
+  s->col_len = (n << log_kept) / comm_world(ctx);
   BJ_TRY(s->lde.alloc(ctx, (size_t)(V + C + T) * s->col_len));
-  BJ_TRY(lde_kept(ctx, d_sigmas, (uint64_t*)s->lde.p, log_n, log_d, V, kept));
-  if (C) BJ_TRY(lde_kept(ctx, d_constants, (uint64_t*)s->lde.p + (size_t)V * s->col_len, log_n, log_d, C, kept));
-  if (T) BJ_TRY(lde_kept(ctx, d_lookup_tables, (uint64_t*)s->lde.p + (size_t)(V + C) * s->col_len, log_n, log_d, T, kept));
+  BJ_TRY(lde_columns(ctx, d_sigmas, (uint64_t*)s->lde.p, log_n, log_kept, V));
+  if (C) BJ_TRY(lde_columns(ctx, d_constants, (uint64_t*)s->lde.p + (size_t)V * s->col_len, log_n, log_kept, C));
+  if (T) BJ_TRY(lde_columns(ctx, d_lookup_tables, (uint64_t*)s->lde.p + (size_t)(V + C) * s->col_len, log_n, log_kept, T));
   for (uint32_t j = 0; j < V + C + T; j++) s->tree.cols.push_back(s->col(j));
   BJ_TRY(oracle_build(ctx, s->tree, n << log_l, circuit->merkle_tree_cap_size, circuit->tree_hasher, circuit->fri_lde_factor));
   if (s->compact) {
@@ -713,7 +711,7 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   const u64 nb = n >> split;                                             // rows of one unit
   const bool compact = setup->compact, streamed = setup->streamed;
   const u64 Qn = n * Q;  // compact plan: elements of a setup / witness / stage-2 column kept on the device (cosets [0, Q))
-  const uint32_t kept = streamed ? L : 0;  // streamed plan: those columns are evaluated on the cosets [0, L) only
+  const uint32_t log_kept = streamed ? log_l : log_d;  // streamed plan: those columns are evaluated on the cosets [0, L) only
   const u64 nK = streamed ? nL : nD;      // stride of those columns on the resident and streamed plans
   if (setup->col_len != (compact ? Qn : nK)) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: the setup was built with a different shard");
   const uint32_t chunk = setup->chunk;  // compact plan: natural-order columns recomputed at a time
@@ -768,11 +766,11 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     if (lk) BJ_TRY(lde_grouped(ctx, w_groups, d_multiplicities, 1, log_n, log_d, &m_col));
   } else {
     BJ_TRY(w_lde.alloc(ctx, (size_t)V * nK));
-    BJ_TRY(lde_kept(ctx, d_variables, (uint64_t*)w_lde.p, log_n, log_d, V, kept));
+    BJ_TRY(lde_columns(ctx, d_variables, (uint64_t*)w_lde.p, log_n, log_kept, V));
     for (uint32_t j = 0; j < V; j++) w_cols[j] = (const uint64_t*)w_lde.p + (size_t)j * nK;
     if (lk) {
       BJ_TRY(m_lde.alloc(ctx, nK));
-      BJ_TRY(lde_kept(ctx, d_multiplicities, (uint64_t*)m_lde.p, log_n, log_d, 1, kept));
+      BJ_TRY(lde_columns(ctx, d_multiplicities, (uint64_t*)m_lde.p, log_n, log_kept, 1));
       m_col = (const uint64_t*)m_lde.p;
     }
   }
@@ -829,13 +827,14 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     BJ_TRY(lde_grouped(ctx, s2_groups, (const uint64_t*)st2.p, n_s2, log_n, log_d, s2_cols.data()));
   } else {
     BJ_TRY(s2_lde.alloc(ctx, (size_t)n_s2 * nK));
-    BJ_TRY(lde_kept(ctx, (const uint64_t*)st2.p, (uint64_t*)s2_lde.p, log_n, log_d, n_s2, kept));
+    BJ_TRY(lde_columns(ctx, (const uint64_t*)st2.p, (uint64_t*)s2_lde.p, log_n, log_kept, n_s2));
     for (uint32_t j = 0; j < n_s2; j++) s2_cols[j] = (const uint64_t*)s2_lde.p + (size_t)j * nK;
   }
   // a row block of a split shard does not hold z(omega x) (another block of the coset does).  On a unit with shift sigma,
-  // z(omega x) is the LDE of z on the shift sigma * omega in the same row order: two more columns (c0, c1 of z)
+  // z(omega x) is the LDE of z on the shift sigma * omega in the same row order: two more columns (c0, c1 of z).  The
+  // streamed plan evaluates them one unit at a time with the quotient's other columns.
   DevMem z_next;
-  if (split && ctx->shard.local_units(Q)) {
+  if (split && !streamed && ctx->shard.local_units(Q)) {
     BJ_TRY(z_next.alloc(ctx, 2 * nD));
     BJ_TRY(bj_lde_next_row(ctx, (const uint64_t*)st2.p, n, (uint64_t*)z_next.p, log_n, log_d, 2, 0));
   }
@@ -890,6 +889,7 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   struct QuotientCols {
     std::vector<const uint64_t*> w, sigma, consts, tables, s2;
     const uint64_t* m;
+    const uint64_t *z_next0, *z_next1;  // split shard: z(omega x) on the same points
   };
   auto quotient_terms = [&](const QuotientCols& k, u64 n_points, uint64_t* o0, uint64_t* o1) -> int32_t {
     if (lk) {
@@ -909,8 +909,8 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
       BJ_TRY(bj_non_residues_for_copy_permutation(n, V, nr.data()));
       const uint64_t b[2] = {beta.c0, beta.c1}, g[2] = {gamma.c0, gamma.c1};
       if (split)
-        BJ_TRY(bj_quotient_copy_permutation_with_z_next(ctx, k.w.data(), k.sigma.data(), V, nr.data(), k.s2[0], k.s2[1], (const uint64_t*)z_next.p,
-                                                        (const uint64_t*)z_next.p + nD, n_partial ? k.s2.data() + 2 : nullptr, b, g,
+        BJ_TRY(bj_quotient_copy_permutation_with_z_next(ctx, k.w.data(), k.sigma.data(), V, nr.data(), k.s2[0], k.s2[1], k.z_next0,
+                                                        k.z_next1, n_partial ? k.s2.data() + 2 : nullptr, b, g,
                                                         powers.data() + 2 * (size_t)(n_lk_terms + n_gate_terms), log_n, log_d, log_q, Q, o0, o1));
       else
         BJ_TRY(bj_quotient_copy_permutation(ctx, k.w.data(), k.sigma.data(), V, nr.data(), k.s2[0], k.s2[1],
@@ -920,37 +920,49 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     return bj_quotient_divide_by_vanishing(ctx, o0, o1, log_n, log_q);
   };
   if (!streamed) {
-    if (nQl) BJ_TRY(quotient_terms({w_cols, sigma_cols, const_cols, table_cols, s2_cols, m_col}, nQl, q0, q1));
+    const uint64_t* zn = (const uint64_t*)z_next.p;
+    if (nQl) BJ_TRY(quotient_terms({w_cols, sigma_cols, const_cols, table_cols, s2_cols, m_col, zn, zn ? zn + nD : nullptr}, nQl, q0, q1));
   } else {
-    // one quotient coset j at a time, under the window of coset j: cosets [0, L) from the kept columns, cosets [L, Q) evaluated
-    // into one coset-sized scratch from the natural-order columns
+    // one local quotient unit k at a time (global unit u: coset u on one GPU or a coset shard, a row block of nb rows of
+    // coset u / B on a split shard), under the window of unit u.  Units of the committed cosets [0, L) come from the kept
+    // columns (their first L * B / world local units), the others are evaluated into one unit-sized scratch from the
+    // natural-order columns; on a split shard the unit's z(omega x) columns go to the scratch too.
+    const CosetShard shard = ctx->shard;
+    const u64 q_units = shard.local_units(Q), kept_units = shard.local_units(L);
     DevMem ev;
-    BJ_TRY(ev.alloc(ctx, (size_t)(2 * V + C + T + (lk ? 1 : 0) + n_s2) * n));
-    for (uint32_t j = 0; j < Q; j++) {
-      QuotientCols k;
+    BJ_TRY(ev.alloc(ctx, (size_t)(2 * V + C + T + (lk ? 1 : 0) + n_s2 + (split ? 2 : 0)) * nb));
+    for (u64 k = 0; k < q_units; k++) {
+      ShardWindow window(ctx, log_q + split, (u32)shard.global_unit(k), split);
+      QuotientCols qc;
       uint64_t* e = (uint64_t*)ev.p;
-      // columns `kept` moved to coset j, or `cnt` natural columns of `nat` evaluated on coset j into the next slots of ev
-      auto coset_j = [&](const std::vector<const uint64_t*>& kept_cols, const uint64_t* nat, uint32_t cnt, std::vector<const uint64_t*>& out) -> int32_t {
+      // columns `kept` moved to unit k, or `cnt` natural columns of `nat` evaluated on unit u into the next slots of ev
+      // (bj_lde under the window: the same coset transform, or fold + row-block transform, as the resident plan's LDE)
+      auto unit_k = [&](const std::vector<const uint64_t*>& kept_cols, const uint64_t* nat, uint32_t cnt, std::vector<const uint64_t*>& out) -> int32_t {
         out.resize(cnt);
-        if (j < L) {
-          for (uint32_t i = 0; i < cnt; i++) out[i] = kept_cols[i] + (size_t)j * n;
+        if (k < kept_units) {
+          for (uint32_t i = 0; i < cnt; i++) out[i] = kept_cols[i] + (size_t)k * nb;
           return BJ_OK;
         }
-        if (cnt) BJ_TRY(bj_lde_cosets(ctx, nat, n, e, log_n, log_d, j, j + 1, cnt, 0));
-        for (uint32_t i = 0; i < cnt; i++) out[i] = e + (size_t)i * n;
-        e += (size_t)cnt * n;
+        if (cnt) BJ_TRY(bj_lde(ctx, nat, n, e, log_n, log_d, cnt, 0));
+        for (uint32_t i = 0; i < cnt; i++) out[i] = e + (size_t)i * nb;
+        e += (size_t)cnt * nb;
         return BJ_OK;
       };
-      BJ_TRY(coset_j(w_cols, d_variables, V, k.w));
-      BJ_TRY(coset_j(sigma_cols, setup->sigmas, V, k.sigma));
-      BJ_TRY(coset_j(const_cols, setup->constants, C, k.consts));
-      BJ_TRY(coset_j(table_cols, setup->tables, T, k.tables));
-      BJ_TRY(coset_j(s2_cols, (const uint64_t*)st2.p, n_s2, k.s2));
+      BJ_TRY(unit_k(w_cols, d_variables, V, qc.w));
+      BJ_TRY(unit_k(sigma_cols, setup->sigmas, V, qc.sigma));
+      BJ_TRY(unit_k(const_cols, setup->constants, C, qc.consts));
+      BJ_TRY(unit_k(table_cols, setup->tables, T, qc.tables));
+      BJ_TRY(unit_k(s2_cols, (const uint64_t*)st2.p, n_s2, qc.s2));
       std::vector<const uint64_t*> mj;
-      if (lk) BJ_TRY(coset_j({m_col}, d_multiplicities, 1, mj));
-      k.m = lk ? mj[0] : nullptr;
-      ShardWindow window(ctx, log_q, j);
-      BJ_TRY(quotient_terms(k, n, q0 + (size_t)j * n, q1 + (size_t)j * n));
+      if (lk) BJ_TRY(unit_k({m_col}, d_multiplicities, 1, mj));
+      qc.m = lk ? mj[0] : nullptr;
+      qc.z_next0 = qc.z_next1 = nullptr;
+      if (split) {
+        BJ_TRY(bj_lde_next_row(ctx, (const uint64_t*)st2.p, n, e, log_n, log_d, 2, 0));
+        qc.z_next0 = e;
+        qc.z_next1 = e + nb;
+      }
+      BJ_TRY(quotient_terms(qc, nb, q0 + (size_t)k * nb, q1 + (size_t)k * nb));
     }
   }
   z_next.release();
@@ -1464,6 +1476,14 @@ int32_t bj_proof_memory_plan(const bj_circuit* circuit, uint32_t world, uint64_t
 }
 
 int32_t bj_proof_memory_plan_streamed(const bj_circuit* circuit, uint32_t world, uint64_t* out) {
+  ProofShape sh;
+  if (!out) return BJ_ERR_INVALID_ARG;
+  BJ_TRY(memory_plan_shape(circuit, world, &sh));
+  *out = world == 1 && streamed_applies(sh) ? plan_bytes(sh, PLAN_STREAMED) : 0;
+  return BJ_OK;
+}
+
+int32_t bj_proof_memory_plan_streamed_sharded(const bj_circuit* circuit, uint32_t world, uint64_t* out) {
   ProofShape sh;
   if (!out) return BJ_ERR_INVALID_ARG;
   BJ_TRY(memory_plan_shape(circuit, world, &sh));

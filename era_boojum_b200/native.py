@@ -127,6 +127,7 @@ SIGNATURES = {
     "bj_setup_free": (None, [_vp]),
     "bj_proof_memory_plan": (_i32, [_vp, _u32, _vp]),
     "bj_proof_memory_plan_streamed": (_i32, [_vp, _u32, _vp]),
+    "bj_proof_memory_plan_streamed_sharded": (_i32, [_vp, _u32, _vp]),
     "bj_setup_is_compact": (_i32, [_vp]),
     "bj_setup_plan": (_i32, [_vp]),
     "bj_setup_memory_plan": (_i32, [_vp, _vp]),

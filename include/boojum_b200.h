@@ -79,10 +79,11 @@ BJ_API const char* bj_last_error(const bj_ctx* ctx);
 BJ_API uint64_t bj_launch_count(const bj_ctx* ctx);
 /* Device-memory limit of the prover driver on this context (bytes; 0, the default: what the device has free when
  * bj_setup_create runs, plus what the context's pool holds without using it).  bj_setup_create compares the memory plans of
- * bj_proof_memory_plan and bj_proof_memory_plan_streamed with it: RESIDENT if that fits, else COMPACT (one GPU, quotient
- * degree < LDE factor), else STREAMED (one GPU, quotient degree > LDE factor), else BJ_ERR_OOM with every applicable byte
- * count in the message and no kernel launched.  With quotient degree = LDE factor only RESIDENT applies.  bj_prove follows
- * the setup's plan and refuses the same way if the limit was lowered below it since. */
+ * bj_proof_memory_plan and bj_proof_memory_plan_streamed(_sharded) with it: RESIDENT if that fits, else COMPACT (one GPU,
+ * quotient degree < LDE factor), else STREAMED (quotient degree > LDE factor, one GPU or sharded), else BJ_ERR_OOM with every
+ * applicable byte count in the message and no kernel launched.  With quotient degree = LDE factor only RESIDENT applies.  On
+ * a sharded context every rank chooses under its own limit; ranks on different plans still return the same proof.  bj_prove
+ * follows the setup's plan and refuses the same way if the limit was lowered below it since. */
 BJ_API int32_t bj_ctx_set_memory_limit(bj_ctx* ctx, uint64_t bytes);
 /* highest device memory the context's pool has had in use (cudaMemPoolAttrUsedMemHigh); reset != 0 restarts the mark.
  * Synchronises.  Memory the library keeps outside the pool (twiddles, coset-power tables, scratch) is not included. */
@@ -502,6 +503,14 @@ BJ_API int32_t bj_proof_memory_plan(const bj_circuit* circuit, uint32_t world, u
  * j >= L evaluated from the natural-order columns into one coset-sized scratch of every column the quotient reads.  Proofs
  * are bit-identical to the resident plan's. */
 BJ_API int32_t bj_proof_memory_plan_streamed(const bj_circuit* circuit, uint32_t world, uint64_t* out);
+/* The STREAMED plan's bytes on each of `world` GPUs (0 when quotient degree <= LDE factor; at world 1 the value of
+ * bj_proof_memory_plan_streamed).  Each rank evaluates the setup, witness and stage-2 columns on its units of the committed
+ * cosets [0, L) only (stride n * L / world) and keeps the natural-order stage-2 columns.  The quotient then runs one of the
+ * rank's units of cosets [0, Q) at a time - the units the resident sharded plan gives the rank: whole cosets on a coset
+ * shard (world <= L), row blocks of n * L / world rows on a split shard - a unit of a committed coset from the kept columns,
+ * any other unit evaluated from the natural-order columns into one unit-sized scratch (with its z(omega x) columns on a
+ * split shard).  The gathered quotient and everything after it are unchanged: every rank returns the single-GPU proof. */
+BJ_API int32_t bj_proof_memory_plan_streamed_sharded(const bj_circuit* circuit, uint32_t world, uint64_t* out);
 /* 1 if bj_setup_create chose the compact plan, 0 otherwise (resident or streamed) */
 BJ_API int32_t bj_setup_is_compact(const bj_setup* setup);
 /* the plan bj_setup_create chose: BJ_PLAN_RESIDENT, BJ_PLAN_COMPACT or BJ_PLAN_STREAMED */
