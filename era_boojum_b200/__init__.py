@@ -17,6 +17,7 @@ No CPU fallback exists: importing this package without the built library raises,
 without a CUDA device raises BoojumError(BJ_ERR_NO_DEVICE).
 """
 import ctypes
+import itertools
 
 import numpy as np
 
@@ -700,6 +701,100 @@ def proof_memory_plan(log_n, num_variables, num_constants, quotient_degree, conf
             "streamed_sharded": int(sharded.value) or None}
 
 
+def witness_slots_bytes(log_n, num_variables, n_slots, max_values=0, lookup=None, world=1):
+    """bj_witness_slots_bytes: device bytes of a set of n_slots witness slots (with a WitnessVec buffer of max_values values and
+    the u32 variables hint when max_values > 0) on each of `world` GPUs, counted from the shapes (no device needed)"""
+    c = native.Circuit()
+    c.log_n, c.num_variables = log_n, num_variables
+    if lookup:
+        c.lookup_width, c.lookup_num_repetitions = lookup["width"], lookup["num_repetitions"]
+    out = ctypes.c_uint64()
+    _ok(lib.bj_witness_slots_bytes(ctypes.byref(c), world, n_slots, max_values, ctypes.byref(out)), "bj_witness_slots_bytes")
+    return int(out.value)
+
+
+def variables_hint_to_u32(hint):
+    """bj_variables_hint_to_u32: reference `Variable`s (bit 63 = placeholder) -> (u32 hint with placeholders 0xFFFFFFFF, 1 + the
+    largest index).  Raises BoojumError(BJ_ERR_INVALID_ARG) on an index >= 2^32 - 1."""
+    h = np.ascontiguousarray(np.asarray(hint).view(np.uint64))
+    out = np.empty(h.shape, np.uint32)
+    need = ctypes.c_uint64()
+    _ok(lib.bj_variables_hint_to_u32(h.ctypes.data_as(ctypes.c_void_p), h.size, out.ctypes.data_as(ctypes.c_void_p), ctypes.byref(need)),
+        "bj_variables_hint_to_u32")
+    return out, int(need.value)
+
+
+def _host_array(a, dtype, n):
+    """(pointer, keep-alive) of a contiguous host array of n elements of dtype: a numpy array or a CPU torch tensor, pinned or
+    pageable (a numpy copy is made only when the layout is not already right)"""
+    if hasattr(a, "data_ptr"):
+        assert not a.is_cuda and a.is_contiguous() and a.element_size() == np.dtype(dtype).itemsize and a.numel() == n
+        return ctypes.c_void_p(a.data_ptr()), a
+    arr = np.ascontiguousarray(a)
+    assert arr.dtype.itemsize == np.dtype(dtype).itemsize and arr.size == n, (arr.dtype, arr.size, n)
+    return arr.ctypes.data_as(ctypes.c_void_p), arr
+
+
+class WitnessSlots:
+    """bj_witness_slots: witness slots of one NativeSetup on the device, filled from host memory on the context's copy stream
+    while proofs run on its stream."""
+
+    def __init__(self, setup, n, max_values=0):
+        self.setup, self.ctx, self.n, self.max_values = setup, setup.ctx, n, max_values
+        _, self.V, _, _, _, _, lookup, _ = setup._vk_args
+        self.lookup = bool(lookup)
+        self.rows = 1 << setup._vk_args[0]
+        self._held = [[] for _ in range(n)]  # host arrays pending uploads may still read (pinned memory is copied asynchronously)
+        h = ctypes.c_void_p()
+        self.ctx._check(lib.bj_witness_slots_create(self.ctx._h, setup._h, n, max_values, ctypes.byref(h)))
+        self._h = h
+
+    def upload(self, slot, variables, multiplicities=None):
+        """bj_witness_upload: variables [V, n] (u64 / int64) and, with a lookup, multiplicities [n]"""
+        pv, kv = _host_array(variables, np.uint64, self.V * self.rows)
+        pm, km = _host_array(multiplicities, np.uint64, self.rows) if multiplicities is not None else (None, None)
+        self.ctx._check(lib.bj_witness_upload(self._h, slot, pv, pm))
+        self._held[slot % self.n].append((kv, km))
+
+    def upload_vec(self, slot, all_values, multiplicities=None):
+        """bj_witness_upload_vec: WitnessVec.all_values (u64) and WitnessVec.multiplicities (u32), gathered through the hint"""
+        nv = len(all_values)
+        pv, kv = _host_array(all_values, np.uint64, nv)
+        nm = len(multiplicities) if multiplicities is not None else 0
+        pm, km = _host_array(multiplicities, np.uint32, nm) if multiplicities is not None else (None, None)
+        self.ctx._check(lib.bj_witness_upload_vec(self._h, slot, pv, nv, pm, nm))
+        self._held[slot % self.n].append((kv, km))
+
+    def columns(self, slot):
+        """bj_witness_slot_columns: a host copy of the slot's columns -> (variables [V, n], multiplicities [n] or None), uint64"""
+        d = ctypes.c_void_p()
+        self.ctx._check(lib.bj_witness_slot_columns(self._h, slot, ctypes.byref(d)))
+        out = np.empty((self.V + self.lookup) * self.rows, np.uint64)
+        self.ctx._check(lib.bj_download(self.ctx._h, out.ctypes.data_as(ctypes.c_void_p), d, out.nbytes))
+        self.ctx.synchronize()
+        v = out[: self.V * self.rows].reshape(self.V, self.rows)
+        return v, (out[self.V * self.rows:] if self.lookup else None)
+
+    def prove(self, slot, timings=None, as_json=True):
+        """bj_prove_slot: the proof of the slot's witness (same bytes as NativeSetup.prove on it)"""
+        h = ctypes.c_void_p()
+        self.ctx._check(lib.bj_prove_slot(self.ctx._h, self.setup._h, self._h, slot, ctypes.byref(h)))
+        self._held[slot % self.n] = []
+        return self.setup._proof_out(h, timings, as_json)
+
+    def close(self):
+        if getattr(self, "_h", None):
+            lib.bj_witness_slots_free(self._h)
+            self._h = None
+            self._held = [[] for _ in range(self.n)]
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 def _circuit(ctx, log_n, num_variables, num_constants, gates, lookup):
     """bj_circuit with the trace shape, the gate programs and the lookup description filled in -> (circuit, keep-alive list)"""
     keep, descs = ctx._gate_descs(gates)
@@ -773,6 +868,57 @@ class NativeSetup:
         h = ctypes.c_void_p()
         self.ctx._check(lib.bj_prove(self.ctx._h, self._h, self.ctx._ptr(variables),
                                      self.ctx._ptr(multiplicities) if multiplicities is not None else None, ctypes.byref(h)))
+        return self._proof_out(h, timings, as_json)
+
+    def attach_variables_hint(self, hint):
+        """bj_setup_attach_variables_hint: the DenseVariablesCopyHint [V, hint_rows] (reference `Variable`s, bit 63 =
+        placeholder; a host array) kept on the device as u32.  prove_stream then takes witnesses as WitnessVec pairs."""
+        h = np.ascontiguousarray(np.asarray(hint).view(np.uint64))
+        assert h.ndim == 2 and h.shape[0] == self._vk_args[1]
+        self.ctx._check(lib.bj_setup_attach_variables_hint(self._h, h.ctypes.data_as(ctypes.c_void_p), h.shape[1]))
+        self.has_hint = True
+
+    has_hint = False
+
+    def witness_slots(self, n=2, max_values=0):
+        """bj_witness_slots_create: n (1 to 4) device slots for witnesses of this setup, plus a WitnessVec buffer of max_values
+        values when max_values > 0"""
+        ws = WitnessSlots(self, n, max_values)
+        self.ctx._children.add(ws)
+        return ws
+
+    def prove_stream(self, witnesses, as_json=True, slots=None):
+        """Proves a stream of witnesses against this setup, yielding the proofs in order.  witnesses: an iterable of
+        (variables [V, n], multiplicities [n] or None) host arrays, or, once a hint is attached, of (all_values,
+        multiplicities as u32) WitnessVec pairs.  With N slots (default: a 2-slot set made here) witness k + N - 1 is uploaded,
+        on the copy stream, before witness k is proved, so the copy overlaps the proof.  Pinned host arrays are read
+        asynchronously and are held until their proof is yielded."""
+        own = slots is None
+        it = iter(witnesses)
+        pending = []
+        try:
+            first = next(it)
+        except StopIteration:
+            return
+        if own:
+            slots = self.witness_slots(2, len(first[0]) if self.has_hint else 0)
+        try:
+            k = 0
+            for w in itertools.chain([first], it):
+                s = k % slots.n
+                slots.upload(s, *w) if not self.has_hint else slots.upload_vec(s, *w)
+                pending.append(s)
+                k += 1
+                if len(pending) == slots.n:
+                    yield slots.prove(pending.pop(0), as_json=as_json)
+            while pending:
+                yield slots.prove(pending.pop(0), as_json=as_json)
+        finally:
+            if own:
+                slots.close()
+
+    def _proof_out(self, h, timings, as_json):
+        """a bj_proof handle -> the proof as a dict or JSON text (the handle is freed)"""
         try:
             need = ctypes.c_size_t()
             _ok(lib.bj_proof_to_json(h, None, 0, ctypes.byref(need)))

@@ -167,6 +167,10 @@ int32_t bj_ctx_destroy(bj_ctx* ctx) {
   if (!ctx) return BJ_OK;
   bj::DeviceGuard device_guard(ctx);
   cudaStreamSynchronize(ctx->stream);
+  if (ctx->witness_stream) {  // uploads of witness slot sets still in flight finish before the memory goes
+    cudaStreamSynchronize(ctx->witness_stream);
+    cudaStreamDestroy(ctx->witness_stream);
+  }
   if (ctx->tw_fwd) cudaFree(ctx->tw_fwd);
   if (ctx->tw_inv) cudaFree(ctx->tw_inv);
   for (auto& e : ctx->pow_cache) {

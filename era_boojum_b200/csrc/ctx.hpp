@@ -113,6 +113,8 @@ struct bj_ctx {
   cudaEvent_t ev_up[3] = {}, ev_done[3] = {}, ev_down[3] = {};
   void* host_ring = nullptr;
   size_t host_ring_bytes = 0;
+  // witness slot sets (witness_stream.cu): the copy stream their uploads run on, created by the first slot set
+  cudaStream_t witness_stream = nullptr;
   void* param_arena = nullptr;  // bump arena for small per-call parameter blocks
   size_t param_off = 0;
   uint64_t launches = 0;  // kernels launched by this library through this context

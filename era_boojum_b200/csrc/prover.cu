@@ -487,6 +487,11 @@ struct bj_setup {
   uint32_t chunk = 2;         // compact plan: natural-order columns recomputed at a time
   uint64_t pool_bytes = 0, outside_pool_bytes = 0;  // the chosen plan (with its chunk): pool peak, library reserve
   uint64_t chosen_bytes() const { return pool_bytes + outside_pool_bytes; }
+  // bj_setup_attach_variables_hint (witness_stream.cu): DenseVariablesCopyHint as u32 [V][hint_rows], 0xFFFFFFFF = placeholder
+  bj::DevMem vars_hint;
+  uint64_t hint_rows = 0;
+  uint64_t hint_values = 0;  // 1 + the largest index the hint names: an all_values vector needs at least this many values
+  bool has_hint = false;
   const uint64_t* col(uint32_t j) const { return (const uint64_t*)lde.p + (size_t)j * col_len; }
   uint32_t log_l() const {
     uint32_t l = 0;

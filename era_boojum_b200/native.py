@@ -136,6 +136,15 @@ SIGNATURES = {
     "bj_proof_free": (None, [_vp]),
     "bj_proof_to_json": (_i32, [_vp, _vp, _sz, ctypes.POINTER(_sz)]),
     "bj_proof_stage_seconds": (_i32, [_vp, _vp]),
+    "bj_witness_slots_bytes": (_i32, [_vp, _u32, _u32, _u64, _vp]),
+    "bj_witness_slots_create": (_i32, [_vp, _vp, _u32, _u64, _pp]),
+    "bj_witness_slots_free": (None, [_vp]),
+    "bj_witness_upload": (_i32, [_vp, _u32, _vp, _vp]),
+    "bj_setup_attach_variables_hint": (_i32, [_vp, _vp, _u64]),
+    "bj_variables_hint_to_u32": (_i32, [_vp, _u64, _vp, _vp]),
+    "bj_witness_upload_vec": (_i32, [_vp, _u32, _vp, _u64, _vp, _u64]),
+    "bj_prove_slot": (_i32, [_vp, _vp, _vp, _u32, _pp]),
+    "bj_witness_slot_columns": (_i32, [_vp, _u32, _pp]),
     "bj_check_satisfied": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bj_lookup_multiplicities": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp]),
     "bj_selftest_field": (_i32, [_vp, _u64, _u64, _vp]),

@@ -41,11 +41,23 @@ def sha_shaped_gates(num_variables=60):
             g(REDUCTION4, num_variables // 5, [False])]
 
 
-def generate(ctx, log_n, num_variables=60, seed=0, lookup=False):
+def _witness_rnd(rnd, dev, witness_seed):
+    """the draw of the free witness values: from the circuit's own generator, or, with a witness seed, from a second one - so
+    circuits of one seed and different witness seeds share sigmas, constants and tables (one setup, many witnesses)"""
+    if witness_seed is None:
+        return rnd
+    import torch
+    gen = torch.Generator(device=dev)
+    gen.manual_seed(witness_seed)
+    return lambda shape, hi: torch.randint(0, hi, shape, dtype=torch.int64, device=dev, generator=gen)
+
+
+def generate(ctx, log_n, num_variables=60, seed=0, lookup=False, witness_seed=None):
     """Returns (variables [V, n], sigmas [V, n], constants [C, n], gates, quotient_degree) as int64 CUDA tensors, C = 6.
     With lookup=True (the bench's 8 sub-arguments of width 4 with a shared table id in a constant column,
     src/gadgets/sha256/mod.rs:340-346): V grows by 32 specialised lookup columns, C = 7 (column 6 = table id) and a sixth
-    return value dict(width, num_repetitions, variables_offset, table_id_column, tables [5, n], multiplicities [n])."""
+    return value dict(width, num_repetitions, variables_offset, table_id_column, tables [5, n], multiplicities [n]).
+    witness_seed: draw the free witness values from their own generator (see _witness_rnd)."""
     torch = ctx._torch
     n_gp = num_variables
     V, n, C = num_variables, 1 << log_n, 6
@@ -53,17 +65,18 @@ def generate(ctx, log_n, num_variables=60, seed=0, lookup=False):
     gen = torch.Generator(device=dev)
     gen.manual_seed(seed)
     rnd = lambda shape, hi: torch.randint(0, hi, shape, dtype=torch.int64, device=dev, generator=gen)
+    wrnd = _witness_rnd(rnd, dev, witness_seed)
     gates = sha_shaped_gates(V)
     n_fma, n_red = V // 4, V // 5
     kind = rnd((n,), 3)                     # 0 = constant allocator, 1 = fma, 2 = reduction
     is_ca, is_fma, is_red = kind == 0, kind == 1, kind == 2
-    variables = rnd((V, n), 1 << 20)
+    variables = wrnd((V, n), 1 << 20)
     constants = torch.zeros((C, n), dtype=torch.int64, device=dev)
     # selector tree: column 0 splits {reduction | others}, column 1 splits {fma | constant allocator}
     constants[0] = (~is_red).to(torch.int64)
     # ---- fma rows: d_k = c0 * a_k * b_k + c1 * c_k, c1 = 1, c_k = d_{k-1}
     c0 = rnd((n,), 1 << 10) + 1
-    fma = rnd((V, n), 1 << 20)
+    fma = wrnd((V, n), 1 << 20)
     for k in range(n_fma):
         if k > 0:
             fma[4 * k + 2] = fma[4 * k - 1]
@@ -71,7 +84,7 @@ def generate(ctx, log_n, num_variables=60, seed=0, lookup=False):
     # ---- reduction rows: r_k = sum_i c_i * v_{k,i}, v_{k,0} = r_{k-1}
     rc = rnd((4, n), 1 << 8)
     rc[0] = 1                               # the chained input enters with coefficient 1 so values grow additively
-    red = rnd((V, n), 1 << 16)
+    red = wrnd((V, n), 1 << 16)
     for k in range(n_red):
         if k > 0:
             red[5 * k] = red[5 * k - 1]
@@ -119,7 +132,7 @@ def generate(ctx, log_n, num_variables=60, seed=0, lookup=False):
     tables[2, :T] = idx ^ 0x5555
     tables[3, :T] = 7 * idx + 1
     tables[4, :T] = 1                      # table id column
-    picks = rnd((nsub, n), T)
+    picks = wrnd((nsub, n), T)
     lk_cols = torch.stack([tables[j][picks[i]] for i in range(nsub) for j in range(width)])      # [32, n]
     mult = torch.bincount(picks.reshape(-1), minlength=n).to(torch.int64)
     table_id_const = torch.ones((1, n), dtype=torch.int64, device=dev)
@@ -185,7 +198,7 @@ PRODUCTION_SELECTOR_PATHS = [
 ]
 
 
-def generate_production_shaped(ctx, log_n, seed=0):
+def generate_production_shaped(ctx, log_n, seed=0, witness_seed=None):
     """A circuit with the GEOMETRY of the reference's vk.json / proof.json fixture (a zkSync recursion-layer circuit): 130
     general-purpose columns with the 11 evaluators above behind its 6-level selector tree, 8 lookup sub-arguments of width 3
     over specialised columns (table id in constant column 7), a BooleanConstraintGate on one specialised column - 155 columns
@@ -193,7 +206,7 @@ def generate_production_shaped(ctx, log_n, seed=0):
     public inputs.  Rows are NopGate rows (any values), ConstantsAllocator rows, FMA rows and Reduction rows (chained by copy
     constraints, as in generate()); the other evaluators are selected on no row but are EVALUATED on every point, which is
     what the prover's cost depends on.  Returns dict(variables, sigmas, constants, gates, quotient_degree, lookup,
-    public_inputs)."""
+    public_inputs).  witness_seed: draw the free witness values from their own generator (see _witness_rnd)."""
     from . import gate_library as GL
     torch = ctx._torch
     GP, W, NSUB = 130, 3, 8
@@ -202,6 +215,7 @@ def generate_production_shaped(ctx, log_n, seed=0):
     gen = torch.Generator(device=dev)
     gen.manual_seed(seed)
     rnd = lambda shape, hi: torch.randint(0, hi, shape, dtype=torch.int64, device=dev, generator=gen)
+    wrnd = _witness_rnd(rnd, dev, witness_seed)
     gp_gates = [GL.CONSTANT_ALLOCATOR, GL.U8X4_FMA, GL.poseidon2_flattened_gate(GP, 0), GL.DOT_PRODUCT4, GL.ZERO_CHECK, GL.FMA,
                 GL.UINTX_ADD, GL.SELECTION, GL.PARALLEL_SELECTION4, GL.NOP, GL.REDUCTION4]
     # specialised-column gates come first in the quotient (prover.rs:608-625), then the general-purpose ones in registration order
@@ -212,16 +226,16 @@ def generate_production_shaped(ctx, log_n, seed=0):
     n_fma, n_red, n_ca = GP // 4, GP // 5, 4
     kind = rnd((n,), 4)                     # 0 = nop, 1 = constants allocator, 2 = fma, 3 = reduction
     is_ca, is_fma, is_red = kind == 1, kind == 2, kind == 3
-    gp = rnd((GP, n), 1 << 20)
+    gp = wrnd((GP, n), 1 << 20)
     c0 = rnd((n,), 1 << 10) + 1
-    fma = rnd((GP, n), 1 << 20)
+    fma = wrnd((GP, n), 1 << 20)
     for k in range(n_fma):                  # d_k = c0 * a_k * b_k + 1 * c_k, c_k = d_{k-1}
         if k > 0:
             fma[4 * k + 2] = fma[4 * k - 1]
         fma[4 * k + 3] = c0 * fma[4 * k] * fma[4 * k + 1] + fma[4 * k + 2]
     rc = rnd((4, n), 1 << 8)
     rc[0] = 1
-    red = rnd((GP, n), 1 << 16)
+    red = wrnd((GP, n), 1 << 16)
     for k in range(n_red):                  # r_k = sum_i c_i * v_{k,i}, v_{k,0} = r_{k-1}
         if k > 0:
             red[5 * k] = red[5 * k - 1]
@@ -251,10 +265,10 @@ def generate_production_shaped(ctx, log_n, seed=0):
     tables[1, :T] = idx * idx + 3
     tables[2, :T] = idx ^ 0x5555
     tables[3, :T] = 1
-    picks = rnd((NSUB, n), T)
+    picks = wrnd((NSUB, n), T)
     lk_cols = torch.stack([tables[j][picks[i]] for i in range(NSUB) for j in range(W)])
     mult = torch.bincount(picks.reshape(-1), minlength=n).to(torch.int64)
-    boolean = rnd((1, n), 2)
+    boolean = wrnd((1, n), 2)
     variables = torch.cat([gp, lk_cols, boolean], dim=0)
     # sigmas: identity k_j * omega^i, then the chained cells of fma / reduction rows swapped
     ks = ctx.non_residues_for_copy_permutation(n, V)

@@ -532,6 +532,51 @@ BJ_API int32_t bj_proof_to_json(const bj_proof* proof, char* buf, size_t capacit
 /* wall-clock seconds of the six stages (witness, stage 2, quotient, openings, DEEP+FRI, queries), device work included */
 BJ_API int32_t bj_proof_stage_seconds(const bj_proof* proof, double out[6]);
 
+/* ---- repeated proving: a stream of witnesses against one setup (prove_from_witness_vec_and_precomputations,
+ *      src/cs/implementations/convenience.rs:159-195) ----
+ * A witness slot set holds n_slots (1 to 4) witnesses on the device, each in the layout bj_prove reads: [V][n] variables, then
+ * n multiplicities when the circuit has a lookup.  Uploads run on a copy stream of the context (created by the first slot set),
+ * so the upload of the next witness overlaps the running proof; bj_prove_slot makes the context's stream wait for the slot's
+ * upload and runs bj_prove on it (same proof bytes).  An upload into a slot whose proof has been issued is ordered after that
+ * proof.  Host memory: pinned memory (bj_alloc_host_pinned, cudaHostRegister) is copied directly - the call returns at once and
+ * the buffer must stay unchanged until bj_prove_slot on that slot has returned; pageable memory is copied through a ring of
+ * four 16 MiB pinned staging chunks on the calling thread - the call returns when the last chunk is staged (it blocks only to
+ * refill a chunk whose copy has not finished) and the buffer may be reused at once.
+ * The slot set allocates once, from the context's pool: n_slots * (V + lookup) * n u64, and with max_values > 0 an all_values
+ * buffer of max_values u64 shared by the slots plus, with a lookup, n u32 multiplicities.  bj_witness_slots_bytes counts those
+ * the way bj_proof_memory_plan counts the proof (host only), and with max_values > 0 the u32 variables hint at its largest
+ * (V * n u32); it is the same on each of `world` GPUs: every rank of a sharded context holds the whole witness.
+ * bj_witness_slots_create refuses with BJ_ERR_OOM, naming both numbers and launching nothing, if the setup's chosen plan plus
+ * those bytes exceed the context's limit (bj_ctx_set_memory_limit, else the limit the setup was planned under).  Free the slot
+ * set before its setup and context (both drain its copy stream).  Argument errors return BJ_ERR_INVALID_ARG with a message
+ * before any launch: another context's setup, a slot out of range, a slot never uploaded, a witness vector without hint or
+ * buffer, a lookup without multiplicities. */
+typedef struct bj_witness_slots bj_witness_slots;
+BJ_API int32_t bj_witness_slots_bytes(const bj_circuit* circuit, uint32_t world, uint32_t n_slots, uint64_t max_values, uint64_t* out);
+BJ_API int32_t bj_witness_slots_create(bj_ctx* ctx, const bj_setup* setup, uint32_t n_slots, uint64_t max_values, bj_witness_slots** out);
+BJ_API void bj_witness_slots_free(bj_witness_slots* slots);
+/* columns from host memory into a slot: h_variables [V][n], h_multiplicities n values (NULL without a lookup) */
+BJ_API int32_t bj_witness_upload(bj_witness_slots* slots, uint32_t slot, const uint64_t* h_variables, const uint64_t* h_multiplicities);
+/* DenseVariablesCopyHint (witness.rs:325-385) in the Variable encoding, [V][hint_rows], hint_rows <= n: kept on the device as u32
+ * with placeholders as 0xFFFFFFFF (half the bytes).  BJ_ERR_INVALID_ARG if an index is >= 2^32 - 1.  Synchronises. */
+BJ_API int32_t bj_setup_attach_variables_hint(bj_setup* setup, const uint64_t* h_hint, uint64_t hint_rows);
+/* the host conversion it uses: n Variables -> u32 (placeholder 0xFFFFFFFF); *h_values_needed (may be NULL) = 1 + the largest
+ * index, 0 if none.  BJ_ERR_INVALID_ARG on an index >= 2^32 - 1. */
+BJ_API int32_t bj_variables_hint_to_u32(const uint64_t* h_hint, uint64_t n, uint32_t* h_out, uint64_t* h_values_needed);
+/* WitnessVec (witness.rs:32-40): all_values (n_values <= max_values, at least what the hint names) and the u32 multiplicities
+ * (1 to n of them, widened and zero-padded to n as witness.rs:493-520 does), gathered into the slot on the copy stream:
+ * variables[c][row] = all_values[hint[c][row]] for row < hint_rows, zero for placeholders and later rows (bj_materialize_columns'
+ * result).  The next upload refills all_values after that gather. */
+BJ_API int32_t bj_witness_upload_vec(bj_witness_slots* slots, uint32_t slot, const uint64_t* h_all_values, uint64_t n_values,
+                                     const uint32_t* h_multiplicities, uint64_t n_multiplicities);
+/* bj_prove on the slot's witness, ordered after its upload; a sharded context runs the sharded driver (every rank uploads the
+ * same witness into its own slot set) */
+BJ_API int32_t bj_prove_slot(bj_ctx* ctx, const bj_setup* setup, bj_witness_slots* slots, uint32_t slot, bj_proof** out);
+/* the slot's device columns (variables [V][n], then the multiplicities), e.g. for bj_check_satisfied: the context's stream is
+ * made to wait for the slot's upload, so work queued on it afterwards reads the whole witness.  Valid until the next upload into
+ * the slot is issued. */
+BJ_API int32_t bj_witness_slot_columns(bj_witness_slots* slots, uint32_t slot, uint64_t** d_columns);
+
 /* ---- satisfiability check: CSReferenceAssembly::check_if_satisfied (src/cs/implementations/satisfiability_test.rs:15-353) ----
  * Checks a witness against its circuit exactly (no random challenge) on the trace domain, from the natural-order device columns
  * bj_setup_create and bj_prove take, with no setup (no LDE, no tree).  It reads log_n, num_variables, num_constants,
