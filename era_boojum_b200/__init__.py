@@ -248,6 +248,12 @@ class Context:
         memory, with every applicable plan's byte count) if none does."""
         self._check(lib.bj_ctx_set_memory_limit(self._h, int(nbytes)))
 
+    def allow_recompute_plan(self, allow=True):
+        """bj_ctx_allow_recompute_plan: with allow, native_setup falls back to the recompute plan (one GPU, any quotient degree;
+        no coset of the setup, witness or stage-2 columns kept, every reader rebuilds the cosets it needs, so slower) when no
+        other plan fits under the limit.  Off by default; a sharded context ignores it."""
+        self._check(lib.bj_ctx_allow_recompute_plan(self._h, int(bool(allow))))
+
     def memory_high_water(self, reset=False):
         """bj_ctx_memory_high_water: the highest device memory the context's pool has had in use (bytes)"""
         v = ctypes.c_uint64()
@@ -682,9 +688,11 @@ class Comm:
 def proof_memory_plan(log_n, num_variables, num_constants, quotient_degree, config, lookup=None, world=1):
     """bj_proof_memory_plan: device bytes of native_setup + prove at their peak on each of `world` GPUs, counted from the
     shapes (no device needed).  -> dict(resident=bytes, compact=bytes or None, streamed=bytes or None,
-    streamed_sharded=bytes or None), None where the plan does not apply (compact: one GPU with quotient degree < LDE factor;
-    streamed: one GPU with quotient degree > LDE factor, bj_proof_memory_plan_streamed; streamed_sharded: the streamed plan on
-    each of `world` GPUs, quotient degree > LDE factor, bj_proof_memory_plan_streamed_sharded)."""
+    streamed_sharded=bytes or None, recompute=bytes or None), None where the plan does not apply (compact: one GPU with
+    quotient degree < LDE factor; streamed: one GPU with quotient degree > LDE factor, bj_proof_memory_plan_streamed;
+    streamed_sharded: the streamed plan on each of `world` GPUs, quotient degree > LDE factor,
+    bj_proof_memory_plan_streamed_sharded; recompute: one GPU, any quotient degree, bj_proof_memory_plan_recompute, chosen only
+    after Context.allow_recompute_plan)."""
     c = native.Circuit()
     c.log_n, c.num_variables, c.num_constants, c.quotient_degree = log_n, num_variables, num_constants, quotient_degree
     c.fri_lde_factor, c.merkle_tree_cap_size = config.fri_lde_factor, config.merkle_tree_cap_size
@@ -697,8 +705,10 @@ def proof_memory_plan(log_n, num_variables, num_constants, quotient_degree, conf
     _ok(lib.bj_proof_memory_plan_streamed(ctypes.byref(c), world, ctypes.byref(streamed)), "bj_proof_memory_plan_streamed")
     sharded = ctypes.c_uint64()
     _ok(lib.bj_proof_memory_plan_streamed_sharded(ctypes.byref(c), world, ctypes.byref(sharded)), "bj_proof_memory_plan_streamed_sharded")
+    recompute = ctypes.c_uint64()
+    _ok(lib.bj_proof_memory_plan_recompute(ctypes.byref(c), world, ctypes.byref(recompute)), "bj_proof_memory_plan_recompute")
     return {"resident": int(out[0]), "compact": int(out[1]) or None, "streamed": int(streamed.value) or None,
-            "streamed_sharded": int(sharded.value) or None}
+            "streamed_sharded": int(sharded.value) or None, "recompute": int(recompute.value) or None}
 
 
 def witness_slots_bytes(log_n, num_variables, n_slots, max_values=0, lookup=None, world=1):
@@ -841,14 +851,16 @@ class NativeSetup:
 
     @property
     def plan(self):
-        """the memory plan bj_setup_create chose (bj_setup_plan): "resident", "compact" or "streamed\""""
+        """the memory plan bj_setup_create chose (bj_setup_plan): "resident", "compact", "streamed" or "recompute\""""
         k = lib.bj_setup_plan(self._h)
         _ok(min(k, 0), "bj_setup_plan")
-        return {native.PLAN_RESIDENT: "resident", native.PLAN_COMPACT: "compact", native.PLAN_STREAMED: "streamed"}[k]
+        return {native.PLAN_RESIDENT: "resident", native.PLAN_COMPACT: "compact", native.PLAN_STREAMED: "streamed",
+                native.PLAN_RECOMPUTE: "recompute"}[k]
 
     def memory_plan(self):
         """bj_setup_memory_plan: the chosen plan -> dict(pool=peak pool bytes of setup + prove, outside_pool=bound on the
-        library's other device memory, chunk=columns the compact plan recomputes at a time, 0 on the resident plan)"""
+        library's other device memory, chunk=columns the compact or recompute plan recomputes at a time, 0 on the resident and
+        streamed plans)"""
         out = (ctypes.c_uint64 * 3)()
         _ok(lib.bj_setup_memory_plan(self._h, out), "bj_setup_memory_plan")
         return {"pool": int(out[0]), "outside_pool": int(out[1]), "chunk": int(out[2])}

@@ -138,6 +138,7 @@ struct bj_ctx {
   bj::CosetShard shard;  // bj_ctx_set_coset_shard / bj_ctx_set_domain_shard; default = the whole domain
   uint32_t shard_log_lde = 0;  // LDE factor the shard was declared for (locates the coset bits of flat indices)
   uint64_t memory_limit = 0;   // bj_ctx_set_memory_limit: device bytes a proof may use (0: what is free when the setup is created)
+  bool allow_recompute_plan = false;  // bj_ctx_allow_recompute_plan: bj_setup_create may fall back to the recompute plan (one GPU)
 };
 
 #define BJ_FAIL(ctx, code, msg)          \

@@ -61,6 +61,22 @@ __global__ void __launch_bounds__(128) keccak_node_kernel(const u64* __restrict_
   for (int k = 0; k < 4; k++) next[4 * i + k] = st[k];
 }
 
+// the node levels of a tree over existing leaf hashes (the leaves may have been hashed a slice at a time)
+int32_t merkle_nodes_keccak256(bj_ctx* ctx, const u64* d_leaf_hashes, u64 n_leaves, u32 cap_size, u64* d_nodes) {
+  const u64* prev = d_leaf_hashes;
+  u64 cnt = n_leaves, written = 0;
+  while (cnt > cap_size) {
+    const u64 next = cnt / 2;
+    u64* dst = d_nodes + 4 * written;
+    keccak_node_kernel<<<(unsigned)((next + 127) / 128), 128, 0, ctx->stream>>>(prev, next, dst);
+    BJ_LAUNCH_CHECK(ctx);
+    prev = dst;
+    written += next;
+    cnt = next;
+  }
+  return BJ_OK;
+}
+
 }  // namespace bj
 
 using namespace bj;
@@ -83,17 +99,7 @@ int32_t bj_merkle_build_keccak256(bj_ctx* ctx, const uint64_t* const* h_sources,
   keccak_leaf_kernel<<<(unsigned)((n_leaves + 127) / 128), 128, 0, ctx->stream>>>((const u64* const*)d_src, n_sources, n_leaves, log_epl,
                                                                                   (u64*)d_leaf_hashes);
   BJ_LAUNCH_CHECK(ctx);
-  const u64* prev = (const u64*)d_leaf_hashes;
-  u64 cnt = n_leaves, written = 0;
-  while (cnt > cap_size) {
-    const u64 next = cnt / 2;
-    u64* dst = (u64*)d_nodes + 4 * written;
-    keccak_node_kernel<<<(unsigned)((next + 127) / 128), 128, 0, ctx->stream>>>(prev, next, dst);
-    BJ_LAUNCH_CHECK(ctx);
-    prev = dst;
-    written += next;
-    cnt = next;
-  }
+  if (n_leaves > cap_size) BJ_TRY(merkle_nodes_keccak256(ctx, (const u64*)d_leaf_hashes, n_leaves, cap_size, (u64*)d_nodes));
   return BJ_OK;
 }
 

@@ -58,6 +58,32 @@ struct Oracle {
   std::vector<u64> cap;  // host, 4 * cap_size
 };
 
+int32_t merkle_nodes_poseidon2(bj_ctx* ctx, const u64* d_leaf_hashes, u64 n_leaves, u32 cap_size, u64* d_nodes);  // poseidon2.cu
+int32_t merkle_nodes_blake2s(bj_ctx* ctx, const u64* d_leaf_hashes, u64 n_leaves, u32 cap_size, u64* d_nodes);    // blake2s.cu
+int32_t merkle_nodes_keccak256(bj_ctx* ctx, const u64* d_leaf_hashes, u64 n_leaves, u32 cap_size, u64* d_nodes);  // keccak.cu
+
+// the tree hasher's whole build (leaves, then node levels down to the cap) and its node phase alone
+using MerkleBuild = int32_t (*)(bj_ctx*, const uint64_t* const*, uint32_t, uint64_t, uint32_t, uint32_t, uint64_t*, uint64_t*);
+using MerkleNodes = int32_t (*)(bj_ctx*, const u64*, u64, u32, u64*);
+static MerkleBuild merkle_build(u32 hasher) {
+  return hasher == BJ_HASHER_BLAKE2S ? bj_merkle_build_blake2s : hasher == BJ_HASHER_KECCAK256 ? bj_merkle_build_keccak256 : bj_merkle_build_poseidon2;
+}
+static MerkleNodes merkle_nodes(u32 hasher) {
+  return hasher == BJ_HASHER_BLAKE2S ? merkle_nodes_blake2s : hasher == BJ_HASHER_KECCAK256 ? merkle_nodes_keccak256 : merkle_nodes_poseidon2;
+}
+
+// the cap of a built tree, assembled over the ranks of a sharded context
+static int32_t oracle_cap(bj_ctx* ctx, Oracle& o, u32 cap_global, u32 lde_factor) {
+  const u64 n_leaves = o.n_leaves;
+  const u32 cap_size = o.cap_size;
+  std::vector<u64> local(4 * (size_t)cap_size);
+  const u64* src = n_leaves == cap_size ? o.leaf_hashes.p : o.nodes.p + 4 * (n_leaves - 2 * (u64)cap_size);
+  BJ_CUDA(ctx, cudaMemcpyAsync(local.data(), src, sizeof(u64) * 4 * cap_size, cudaMemcpyDeviceToHost, ctx->stream));
+  BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  o.cap.resize(4 * (size_t)cap_global);
+  return comm_assemble_cap(ctx, local.data(), cap_global, lde_factor, o.cap.data());
+}
+
 // n_leaves / cap_size are GLOBAL; on a coset-sharded context the tree covers this rank's cosets (n_leaves / world leaves,
 // cap_size / world local cap nodes - same depth), and o.cap is the assembled global cap (lde_factor locates the cosets).
 static int32_t oracle_build(bj_ctx* ctx, Oracle& o, u64 n_leaves, u32 cap_size, u32 hasher, u32 lde_factor) {
@@ -70,14 +96,47 @@ static int32_t oracle_build(bj_ctx* ctx, Oracle& o, u64 n_leaves, u32 cap_size, 
   if (cap_size == 0 || n_leaves < cap_size) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "prover: oracle smaller than the cap");
   BJ_TRY(o.leaf_hashes.alloc(ctx, 4 * n_leaves));
   BJ_TRY(o.nodes.alloc(ctx, 4 * (n_leaves - cap_size)));
-  BJ_TRY((hasher == BJ_HASHER_BLAKE2S ? bj_merkle_build_blake2s : hasher == BJ_HASHER_KECCAK256 ? bj_merkle_build_keccak256 : bj_merkle_build_poseidon2)(
-      ctx, o.cols.data(), (u32)o.cols.size(), n_leaves, 1, cap_size, (uint64_t*)o.leaf_hashes.p, (uint64_t*)o.nodes.p));
-  std::vector<u64> local(4 * (size_t)cap_size);
-  const u64* src = n_leaves == cap_size ? o.leaf_hashes.p : o.nodes.p + 4 * (n_leaves - 2 * (u64)cap_size);
-  BJ_CUDA(ctx, cudaMemcpyAsync(local.data(), src, sizeof(u64) * 4 * cap_size, cudaMemcpyDeviceToHost, ctx->stream));
-  BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  o.cap.resize(4 * (size_t)cap_global);
-  return comm_assemble_cap(ctx, local.data(), cap_global, lde_factor, o.cap.data());
+  BJ_TRY(merkle_build(hasher)(ctx, o.cols.data(), (u32)o.cols.size(), n_leaves, 1, cap_size, (uint64_t*)o.leaf_hashes.p, (uint64_t*)o.nodes.p));
+  return oracle_cap(ctx, o, cap_global, lde_factor);
+}
+
+// natural-order columns of stride n: `cnt` of them from `p`
+struct NatSpan {
+  const uint64_t* p;
+  u32 cnt;
+};
+
+// recompute plan (one GPU): the tree of oracle_build over the LDE at factor L of the spans' columns, built one committed coset
+// at a time.  Coset j is leaves [j n, (j + 1) n) (leaf t = j * n + row): its columns are evaluated into an n-row scratch per
+// column (bj_lde_cosets, the transforms of bj_lde), its leaves hashed into their slice, and the node levels are built once
+// the leaf array is complete, so the tree is bit-identical.  o.cols are the natural columns (they give the row length).
+static int32_t oracle_build_by_coset(bj_ctx* ctx, Oracle& o, const std::vector<NatSpan>& spans, u32 log_n, u32 log_l, u32 cap_size, u32 hasher) {
+  const u64 n = 1ull << log_n, n_leaves = n << log_l;
+  o.cols.clear();
+  for (const NatSpan& sp : spans)
+    for (u32 i = 0; i < sp.cnt; i++) o.cols.push_back(sp.p + (size_t)i * n);
+  o.n_leaves = n_leaves;
+  o.cap_size = cap_size;
+  if (cap_size == 0 || n_leaves < cap_size) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "prover: oracle smaller than the cap");
+  BJ_TRY(o.leaf_hashes.alloc(ctx, 4 * n_leaves));
+  {
+    DevMem ev;
+    BJ_TRY(ev.alloc(ctx, o.cols.size() * n));
+    std::vector<const uint64_t*> on_coset(o.cols.size());
+    for (size_t i = 0; i < on_coset.size(); i++) on_coset[i] = (const uint64_t*)ev.p + i * n;
+    for (u32 j = 0; j < (1u << log_l); j++) {
+      size_t c0 = 0;
+      for (const NatSpan& sp : spans) {
+        if (sp.cnt) BJ_TRY(bj_lde_cosets(ctx, sp.p, n, (uint64_t*)ev.p + c0 * n, log_n, log_l, j, j + 1, sp.cnt, 0));
+        c0 += sp.cnt;
+      }
+      // the leaf phase alone: a tree of n leaves whose cap is its leaves
+      BJ_TRY(merkle_build(hasher)(ctx, on_coset.data(), (u32)on_coset.size(), n, 1, (u32)n, (uint64_t*)o.leaf_hashes.p + 4 * (size_t)j * n, nullptr));
+    }
+  }
+  BJ_TRY(o.nodes.alloc(ctx, 4 * (n_leaves - cap_size)));
+  BJ_TRY(merkle_nodes(hasher)(ctx, o.leaf_hashes.p, n_leaves, cap_size, o.nodes.p));
+  return oracle_cap(ctx, o, cap_size, 1u << log_l);
 }
 
 // LDE of trace-domain columns (Lagrange values, natural order) onto this context's cosets.  One GPU: bj_lde.  Sharded: the
@@ -264,16 +323,24 @@ struct QueryAnswer {
 // cosets [L, Q) are read by the quotient alone, which evaluates every column it reads onto one such coset at a time into a
 // coset-sized scratch, from the natural-order columns (the stage-2 ones are kept for it).  On a sharded context each rank
 // keeps its units of the committed cosets and evaluates its own units of cosets [L, Q), one unit (a coset, or a row block
-// of one on a split shard, with its z(omega x) columns) at a time into a unit-sized scratch.  The plan replays the driver's
-// stream-ordered pool allocations in order (pool_peak) and adds what the library keeps outside the pool (library_reserve):
-// twiddles, coset-power tables and the NTT scratch.
-enum MemoryPlan : u32 { PLAN_RESIDENT = BJ_PLAN_RESIDENT, PLAN_COMPACT = BJ_PLAN_COMPACT, PLAN_STREAMED = BJ_PLAN_STREAMED };
+// of one on a split shard, with its z(omega x) columns) at a time into a unit-sized scratch.  RECOMPUTE (one GPU, any Q and
+// L, opt-in) keeps no coset of the setup, witness and stage-2 columns at all: their trees are built one committed coset at a
+// time (oracle_build_by_coset), the quotient runs the streamed plan's unit loop with no kept unit, the openings rebuild coset
+// 0 and DEEP and the queries cosets [0, L), all from the natural-order columns a chunk at a time.  The plan replays the
+// driver's stream-ordered pool allocations in order (pool_peak) and adds what the library keeps outside the pool
+// (library_reserve): twiddles, coset-power tables and the NTT scratch.
+enum MemoryPlan : u32 {
+  PLAN_RESIDENT = BJ_PLAN_RESIDENT,
+  PLAN_COMPACT = BJ_PLAN_COMPACT,
+  PLAN_STREAMED = BJ_PLAN_STREAMED,
+  PLAN_RECOMPUTE = BJ_PLAN_RECOMPUTE
+};
 struct ProofShape {
   u32 V, C, T, W, n_s2, Q, L, log_n, log_l, log_d, log_q, world, split, cap, n_queries, sched_len;
   u32 sched[32];
   u64 n;
   bool lk;
-  u32 nat_cols() const { return V + C + T + W + n_s2; }  // natural-order columns a compact / streamed proof recomputes from
+  u32 nat_cols() const { return V + C + T + W + n_s2; }  // natural-order columns a compact / streamed / recompute proof recomputes from
 };
 
 static int32_t proof_shape(const bj_circuit& c, u32 world, ProofShape* s) {
@@ -312,16 +379,28 @@ struct Ledger {
   void sub(u64 n_u64) { cur -= pool_bytes(n_u64); }
 };
 
-// peak pool bytes of bj_setup_create followed by bj_prove; `chunk`: columns recomputed at a time (compact plan)
+// peak pool bytes of bj_setup_create followed by bj_prove; `chunk`: columns recomputed at a time (compact and recompute plans)
 static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk) {
   Ledger m;
-  const bool compact = plan == PLAN_COMPACT, streamed = plan == PLAN_STREAMED;
+  const bool compact = plan == PLAN_COMPACT, streamed = plan == PLAN_STREAMED, recompute = plan == PLAN_RECOMPUTE;
   const u64 n = s.n, w = s.world, nL = (n << s.log_l) / w, nQ = n << s.log_q, Qn = n * s.Q;
   const u64 nD = streamed ? nL : (n << s.log_d) / w;  // elements of an LDE column as first evaluated
   const u64 leaves = (n << s.log_l) / w, capl = s.cap / w;
   auto tree = [&]() {
     m.add(4 * leaves);
     m.add(4 * (leaves - capl));
+  };
+  auto tree_by_coset = [&](u64 cols) {  // oracle_build_by_coset: leaf hashes, one coset of the columns, then the nodes
+    m.add(4 * leaves);
+    m.add(cols * n);
+    m.sub(cols * n);
+    m.add(4 * (leaves - capl));
+  };
+  auto rebuild_chunks = [&]() {  // for_chunks: the monomials and one coset of a chunk of natural columns
+    m.add((u64)chunk * n);
+    m.add((u64)chunk * n);
+    m.sub((u64)chunk * n);
+    m.sub((u64)chunk * n);
   };
   auto lde_groups = [&](u32 cols) {  // lde_columns on a sharded context: at most two column groups of monomials at once
     if (w == 1 || cols < 2) return;
@@ -332,11 +411,15 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk) {
   };
   const u64 S = s.V + s.C + s.T;
   // bj_setup_create
-  m.add(S * nD);
-  lde_groups(s.V);
-  lde_groups(s.C);
-  lde_groups(s.T);
-  tree();
+  if (recompute) {
+    tree_by_coset(S);
+  } else {
+    m.add(S * nD);
+    lde_groups(s.V);
+    lde_groups(s.C);
+    lde_groups(s.T);
+    tree();
+  }
   if (compact) {
     m.add(S * Qn);
     m.sub(S * nD);
@@ -350,14 +433,16 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk) {
   std::vector<u64> wg = groups(s.V), sg = groups(s.n_s2);
   if (s.lk) wg.push_back(1);
   // round 1
-  if (compact) {
+  if (recompute) {
+    tree_by_coset(s.W);
+  } else if (compact) {
     for (u64 g : wg) m.add(g * nD);
   } else {
     m.add(s.V * nD);
     lde_groups(s.V);
     if (s.lk) m.add(nD);
   }
-  tree();
+  if (!recompute) tree();
   if (compact)
     for (u64 g : wg) {
       m.add(g * Qn);
@@ -365,7 +450,9 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk) {
     }
   // round 2
   m.add(s.n_s2 * n);
-  if (compact) {
+  if (recompute) {
+    tree_by_coset(s.n_s2);
+  } else if (compact) {
     for (u64 g : sg) m.add(g * nD);
   } else {
     m.add(s.n_s2 * nD);
@@ -373,9 +460,10 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk) {
   }
   const u64 zn = s.split && !streamed ? 2 * nD : 0;  // the streamed plan evaluates z(omega x) per unit, into its scratch
   if (zn) m.add(zn);
-  // the compact plan keeps the natural stage-2 columns for DEEP and the queries, the streamed plan for the quotient
-  if (!compact && !streamed) m.sub(s.n_s2 * n);
-  tree();
+  // the compact plan keeps the natural stage-2 columns for DEEP and the queries, the streamed plan for the quotient, the
+  // recompute plan for both
+  if (!compact && !streamed && !recompute) m.sub(s.n_s2 * n);
+  if (!recompute) tree();
   if (compact)
     for (u64 g : sg) {
       m.add(g * Qn);
@@ -385,7 +473,7 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk) {
   m.add(2 * nQ);
   const u64 nQl = ((u64)s.Q << s.split) >= w ? nQ / w : n >> s.split;
   if (w > 1) m.add(2 * std::max<u64>(nQl, 1));
-  if (streamed) {  // one unit of every column the quotient reads (and of z(omega x) on a split shard)
+  if (streamed || recompute) {  // one unit of every column the quotient reads (and of z(omega x) on a split shard)
     const u64 unit = (u64)(s.nat_cols() + (s.split ? 2 : 0)) * (n >> s.split);
     m.add(unit);
     m.sub(unit);
@@ -404,14 +492,11 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk) {
   m.add(2 * (u64)s.Q * nL);
   m.sub(2 * nQ);  // chunks
   tree();
+  // round 4: the recompute plan opens the natural columns on coset 0, rebuilt a chunk at a time
+  if (recompute) rebuild_chunks();
   // round 5
   m.add(2 * nL);
-  if (compact) {  // DEEP on the dropped cosets: monomials + one coset of a chunk of columns
-    m.add((u64)chunk * n);
-    m.add((u64)chunk * n);
-    m.sub((u64)chunk * n);
-    m.sub((u64)chunk * n);
-  }
+  if (compact || recompute) rebuild_chunks();  // DEEP on the cosets not kept
   u64 log_m = s.log_n + s.log_l;
   u32 kmax = 0;
   for (u32 i = 0; i < s.sched_len; i++) {
@@ -435,14 +520,15 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk) {
   }
   m.sub(fft);
   m.sub(fft);
-  // queries: one gather buffer at a time (leaf rows, Merkle paths, FRI leaves); the compact plan then recomputes the rows
-  // of the dropped cosets chunk by chunk
+  // queries: one gather buffer at a time (leaf rows, Merkle paths, FRI leaves; the recompute plan gathers no row of the
+  // setup, witness and stage-2 oracles here); the compact and recompute plans then recompute the rows of the cosets they
+  // do not keep chunk by chunk, gathering all the queries' rows of a chunk at a time
   u32 depth = 0;
   while ((leaves >> depth) > capl) depth++;
-  const u64 row_max = std::max<u64>({S, s.W, s.n_s2, 2 * (u64)s.Q, 4 * (u64)depth, 2ull << kmax});
+  const u64 row_max = std::max<u64>({recompute ? 0 : std::max<u64>({S, s.W, s.n_s2}), 2 * (u64)s.Q, 4 * (u64)depth, 2ull << kmax});
   m.add((u64)s.n_queries * row_max);
   m.sub((u64)s.n_queries * row_max);
-  if (compact) {
+  if (compact || recompute) {
     m.add((u64)chunk * n);
     m.add((u64)chunk * n);
     m.add((u64)s.n_queries * chunk);
@@ -463,6 +549,7 @@ static u64 library_reserve(const ProofShape& s) {
 }
 
 static bool compact_applies(const ProofShape& s) { return s.world == 1 && s.Q < s.L; }
+static bool recompute_applies(const ProofShape& s) { return s.world == 1; }
 static bool streamed_applies(const ProofShape& s) { return s.Q > s.L; }  // on one GPU and on sharded contexts
 
 static u64 plan_bytes(const ProofShape& s, MemoryPlan plan, u32 chunk = 2) { return pool_peak(s, plan, chunk) + library_reserve(s); }
@@ -479,12 +566,13 @@ struct bj_setup {
   uint32_t n_tables = 0;
   bj::DevMem lde;  // [V + C + T][D][n], D = max(L, quotient degree): the tree commits to the first L cosets of every column
   bj::Oracle tree;
-  uint64_t col_len = 0;  // elements of one LDE column held by this context: n * (D / world), n * Q compact, n * (L / world) streamed
+  uint64_t col_len = 0;  // elements of one LDE column held by this context: n * (D / world), n * Q compact, n * (L / world) streamed, 0 recompute
   bool compact = false;   // memory plan chosen by bj_setup_create, followed by bj_prove
   bool streamed = false;
+  bool recompute = false;
   uint64_t limit = 0;    // the device-memory limit the plan was chosen under
-  uint64_t plan[3] = {0, 0, 0};  // resident, compact, streamed (0: the plan does not apply)
-  uint32_t chunk = 2;         // compact plan: natural-order columns recomputed at a time
+  uint64_t plan[4] = {0, 0, 0, 0};  // resident, compact, streamed, recompute (0: the plan does not apply or was not allowed)
+  uint32_t chunk = 2;         // compact and recompute plans: natural-order columns recomputed at a time
   uint64_t pool_bytes = 0, outside_pool_bytes = 0;  // the chosen plan (with its chunk): pool peak, library reserve
   uint64_t chosen_bytes() const { return pool_bytes + outside_pool_bytes; }
   // bj_setup_attach_variables_hint (witness_stream.cu): DenseVariablesCopyHint as u32 [V][hint_rows], 0xFFFFFFFF = placeholder
@@ -545,10 +633,11 @@ static int32_t memory_limit(bj_ctx* ctx, uint64_t* out) {
   return BJ_OK;
 }
 
-static std::string plan_message(const char* who, const uint64_t plan[3], uint64_t limit) {
+static std::string plan_message(const char* who, const uint64_t plan[4], uint64_t limit) {
   std::string m = std::string(who) + ": the proof needs " + std::to_string(plan[0]) + " bytes of device memory resident";
   m += plan[1] ? " and " + std::to_string(plan[1]) + " bytes on the compact plan" : std::string(" (no compact plan: sharded context or quotient degree >= LDE factor)");
   if (plan[2]) m += " and " + std::to_string(plan[2]) + " bytes on the streamed plan";
+  if (plan[3]) m += " and " + std::to_string(plan[3]) + " bytes on the recompute plan";
   return m + ", above the limit of " + std::to_string(limit) + " bytes";
 }
 
@@ -596,32 +685,39 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
   }
   std::unique_ptr<bj_setup> s(new bj_setup());
   {
-    // the memory plan: resident if it fits under the limit, else compact (Q < L, one GPU), else streamed (Q > L); refused
-    // before anything is launched.  On a sharded context every rank chooses under its own limit: the resident and streamed
-    // plans hold the same committed units and run the same collectives, so ranks on different plans still agree
+    // the memory plan: resident if it fits under the limit, else compact (Q < L, one GPU), else streamed (Q > L), else
+    // recompute (one GPU, when the context allows it); refused before anything is launched.  On a sharded context every
+    // rank chooses under its own limit: the resident and streamed plans hold the same committed units and run the same
+    // collectives, so ranks on different plans still agree
     ProofShape sh;
     BJ_TRY(proof_shape(*circuit, comm_world(ctx), &sh));
     s->plan[0] = plan_bytes(sh, PLAN_RESIDENT);
     s->plan[1] = compact_applies(sh) ? plan_bytes(sh, PLAN_COMPACT) : 0;
     s->plan[2] = streamed_applies(sh) ? plan_bytes(sh, PLAN_STREAMED) : 0;
+    s->plan[3] = ctx->allow_recompute_plan && recompute_applies(sh) ? plan_bytes(sh, PLAN_RECOMPUTE) : 0;
     BJ_TRY(memory_limit(ctx, &s->limit));
-    if (s->plan[0] > s->limit && s->plan[2] && s->plan[2] <= s->limit) {
-      s->streamed = true;
-    } else if (s->plan[0] > s->limit) {
-      if (!s->plan[1] || s->plan[1] > s->limit) BJ_FAIL(ctx, BJ_ERR_OOM, plan_message("bj_setup_create", s->plan, s->limit));
-      s->compact = true;
+    auto fits = [&](int k) { return s->plan[k] && s->plan[k] <= s->limit; };
+    if (s->plan[0] > s->limit) {
+      if (fits(2)) s->streamed = true;
+      else if (fits(1)) s->compact = true;
+      else if (fits(3)) s->recompute = true;
+      else BJ_FAIL(ctx, BJ_ERR_OOM, plan_message("bj_setup_create", s->plan, s->limit));
+    }
+    if (s->compact || s->recompute) {
       // wider recompute chunks only save kernel launches: the chunk grows into at most half of the headroom the limit leaves
       // over the plan (the rest is slack for the pool's fragmentation) and stops at 16 columns
-      const uint64_t budget = s->plan[1] + (s->limit - s->plan[1]) / 2;
+      const MemoryPlan kind = s->compact ? PLAN_COMPACT : PLAN_RECOMPUTE;
+      const uint64_t planned = s->plan[s->compact ? 1 : 3];
+      const uint64_t budget = planned + (s->limit - planned) / 2;
       uint32_t lo = 2, hi = std::max<uint32_t>(2, std::min<uint32_t>(16, sh.nat_cols()));
       while (lo < hi) {
         const uint32_t mid = lo + (hi - lo + 1) / 2;
-        if (plan_bytes(sh, PLAN_COMPACT, mid) <= budget) lo = mid;
+        if (plan_bytes(sh, kind, mid) <= budget) lo = mid;
         else hi = mid - 1;
       }
       s->chunk = lo;
     }
-    s->pool_bytes = pool_peak(sh, s->compact ? PLAN_COMPACT : s->streamed ? PLAN_STREAMED : PLAN_RESIDENT, s->chunk);
+    s->pool_bytes = pool_peak(sh, s->compact ? PLAN_COMPACT : s->streamed ? PLAN_STREAMED : s->recompute ? PLAN_RECOMPUTE : PLAN_RESIDENT, s->chunk);
     s->outside_pool_bytes = library_reserve(sh);
   }
   s->ctx = ctx;
@@ -660,7 +756,14 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
   const u64 n = 1ull << log_n;
   // the streamed plan evaluates the committed cosets [0, L) only (this rank's units of them): the LDE at factor L, whose
   // cosets are the first L of the factor-D domain with the same shifts, so the values and trees do not change.  The
-  // quotient recomputes the other cosets from the borrowed natural-order columns.
+  // quotient recomputes the other cosets from the borrowed natural-order columns.  The recompute plan keeps no coset: the
+  // tree is built one coset at a time, and s->tree.cols are the natural-order columns every reader rebuilds its cosets from.
+  if (s->recompute) {
+    BJ_TRY(oracle_build_by_coset(ctx, s->tree, {{d_sigmas, V}, {d_constants, C}, {d_lookup_tables, T}}, log_n, log_l,
+                                 circuit->merkle_tree_cap_size, circuit->tree_hasher));
+    *out = s.release();
+    return BJ_OK;
+  }
   const uint32_t log_kept = s->streamed ? log_l : log_d;
   s->col_len = (n << log_kept) / comm_world(ctx);
   BJ_TRY(s->lde.alloc(ctx, (size_t)(V + C + T) * s->col_len));
@@ -714,12 +817,17 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   const u64 nQl = ctx->shard.local_points(Q, (int)log_n);                 // LOCAL quotient points
   const uint32_t split = ctx->shard.log_split;                            // 2^split row blocks per coset (split domain shard)
   const u64 nb = n >> split;                                             // rows of one unit
-  const bool compact = setup->compact, streamed = setup->streamed;
+  const bool compact = setup->compact, streamed = setup->streamed, recompute = setup->recompute;
   const u64 Qn = n * Q;  // compact plan: elements of a setup / witness / stage-2 column kept on the device (cosets [0, Q))
   const uint32_t log_kept = streamed ? log_l : log_d;  // streamed plan: those columns are evaluated on the cosets [0, L) only
   const u64 nK = streamed ? nL : nD;      // stride of those columns on the resident and streamed plans
-  if (setup->col_len != (compact ? Qn : nK)) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: the setup was built with a different shard");
-  const uint32_t chunk = setup->chunk;  // compact plan: natural-order columns recomputed at a time
+  if (setup->col_len != (compact ? Qn : recompute ? 0 : nK) || (recompute && world > 1))
+    BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: the setup was built with a different shard");
+  const uint32_t chunk = setup->chunk;  // compact and recompute plans: natural-order columns recomputed at a time
+  // the compact plan keeps cosets [0, Q) of the setup, witness and stage-2 columns, the recompute plan none: DEEP and the
+  // query answers rebuild the cosets [first_rebuilt, L) of them from the natural-order columns
+  const uint32_t first_rebuilt = compact ? Q : 0;
+  const u64 Fn = (u64)first_rebuilt * n;
   {
     const uint64_t limit = ctx->memory_limit ? ctx->memory_limit : setup->limit;
     if (setup->chosen_bytes() > limit) BJ_FAIL(ctx, BJ_ERR_OOM, plan_message("bj_prove", setup->plan, limit));
@@ -766,7 +874,12 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   ColumnGroups w_groups;  // compact plan
   std::vector<const uint64_t*> w_cols(V);
   const uint64_t* m_col = nullptr;
-  if (compact) {
+  Oracle w_or;
+  if (recompute) {  // the tree one coset at a time; the columns stand for themselves in natural order from here on
+    BJ_TRY(oracle_build_by_coset(ctx, w_or, {{d_variables, V}, {d_multiplicities, lk ? 1u : 0u}}, log_n, log_l, cap, c.tree_hasher));
+    for (uint32_t j = 0; j < V; j++) w_cols[j] = w_or.cols[j];
+    if (lk) m_col = w_or.cols[V];
+  } else if (compact) {
     BJ_TRY(lde_grouped(ctx, w_groups, d_variables, V, log_n, log_d, w_cols.data()));
     if (lk) BJ_TRY(lde_grouped(ctx, w_groups, d_multiplicities, 1, log_n, log_d, &m_col));
   } else {
@@ -779,10 +892,11 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
       m_col = (const uint64_t*)m_lde.p;
     }
   }
-  Oracle w_or;
-  w_or.cols = w_cols;
-  if (lk) w_or.cols.push_back(m_col);  // variables | witness (none) | multiplicities
-  BJ_TRY(oracle_build(ctx, w_or, n << log_l, cap, c.tree_hasher, L));
+  if (!recompute) {
+    w_or.cols = w_cols;
+    if (lk) w_or.cols.push_back(m_col);  // variables | witness (none) | multiplicities
+    BJ_TRY(oracle_build(ctx, w_or, n << log_l, cap, c.tree_hasher, L));
+  }
   pf->witness_cap = w_or.cap;
   bj_transcript_witness_merkle_tree_cap(tr, (const uint64_t*)w_or.cap.data(), cap);
   if (compact) {
@@ -828,7 +942,11 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   }
   ColumnGroups s2_groups;  // compact plan
   std::vector<const uint64_t*> s2_cols(n_s2);
-  if (compact) {
+  Oracle s2_or;
+  if (recompute) {
+    BJ_TRY(oracle_build_by_coset(ctx, s2_or, {{(const uint64_t*)st2.p, n_s2}}, log_n, log_l, cap, c.tree_hasher));
+    s2_cols = s2_or.cols;
+  } else if (compact) {
     BJ_TRY(lde_grouped(ctx, s2_groups, (const uint64_t*)st2.p, n_s2, log_n, log_d, s2_cols.data()));
   } else {
     BJ_TRY(s2_lde.alloc(ctx, (size_t)n_s2 * nK));
@@ -843,10 +961,12 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     BJ_TRY(z_next.alloc(ctx, 2 * nD));
     BJ_TRY(bj_lde_next_row(ctx, (const uint64_t*)st2.p, n, (uint64_t*)z_next.p, log_n, log_d, 2, 0));
   }
-  if (!compact && !streamed) st2.release();  // the compact plan recomputes cosets [Q, L) of stage 2 from it, the streamed [L, Q)
-  Oracle s2_or;
-  s2_or.cols = s2_cols;
-  BJ_TRY(oracle_build(ctx, s2_or, n << log_l, cap, c.tree_hasher, L));
+  // the compact plan recomputes cosets [Q, L) of stage 2 from it, the streamed [L, Q), the recompute plan every coset
+  if (!compact && !streamed && !recompute) st2.release();
+  if (!recompute) {
+    s2_or.cols = s2_cols;
+    BJ_TRY(oracle_build(ctx, s2_or, n << log_l, cap, c.tree_hasher, L));
+  }
   pf->stage2_cap = s2_or.cap;
   bj_transcript_witness_merkle_tree_cap(tr, (const uint64_t*)s2_or.cap.data(), cap);
   if (compact) {
@@ -872,9 +992,10 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     }
   }
   std::vector<const uint64_t*> const_cols(C), sigma_cols(V), table_cols(T);
-  for (uint32_t j = 0; j < V; j++) sigma_cols[j] = setup->col(j);
-  for (uint32_t j = 0; j < C; j++) const_cols[j] = setup->col(V + j);
-  for (uint32_t j = 0; j < T; j++) table_cols[j] = setup->col(V + C + j);
+  // the setup tree's columns: the kept LDE columns, or on the recompute plan the natural-order ones
+  for (uint32_t j = 0; j < V; j++) sigma_cols[j] = setup->tree.cols[j];
+  for (uint32_t j = 0; j < C; j++) const_cols[j] = setup->tree.cols[V + j];
+  for (uint32_t j = 0; j < T; j++) table_cols[j] = setup->tree.cols[V + C + j];
   DevMem qq, qloc;  // qq: [2][nQ] global (c0 then c1); qloc: this rank's cosets among the first Q
   BJ_TRY(qq.alloc(ctx, 2 * nQ));
   uint64_t* q0 = (uint64_t*)qq.p;
@@ -924,20 +1045,21 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     }
     return bj_quotient_divide_by_vanishing(ctx, o0, o1, log_n, log_q);
   };
-  if (!streamed) {
+  if (!streamed && !recompute) {
     const uint64_t* zn = (const uint64_t*)z_next.p;
     if (nQl) BJ_TRY(quotient_terms({w_cols, sigma_cols, const_cols, table_cols, s2_cols, m_col, zn, zn ? zn + nD : nullptr}, nQl, q0, q1));
   } else {
     // one local quotient unit k at a time (global unit u: coset u on one GPU or a coset shard, a row block of nb rows of
-    // coset u / B on a split shard), under the window of unit u.  Units of the committed cosets [0, L) come from the kept
-    // columns (their first L * B / world local units), the others are evaluated into one unit-sized scratch from the
-    // natural-order columns; on a split shard the unit's z(omega x) columns go to the scratch too.
+    // coset u / B on a split shard), under the window of unit u among the units of the factor-D domain.  On the streamed
+    // plan the units of the committed cosets [0, L) come from the kept columns (their first L * B / world local units); the
+    // others, and every unit on the recompute plan, are evaluated into one unit-sized scratch from the natural-order
+    // columns; on a split shard the unit's z(omega x) columns go to the scratch too.
     const CosetShard shard = ctx->shard;
-    const u64 q_units = shard.local_units(Q), kept_units = shard.local_units(L);
+    const u64 q_units = shard.local_units(Q), kept_units = recompute ? 0 : shard.local_units(L);
     DevMem ev;
     BJ_TRY(ev.alloc(ctx, (size_t)(2 * V + C + T + (lk ? 1 : 0) + n_s2 + (split ? 2 : 0)) * nb));
     for (u64 k = 0; k < q_units; k++) {
-      ShardWindow window(ctx, log_q + split, (u32)shard.global_unit(k), split);
+      ShardWindow window(ctx, log_d + split, (u32)shard.global_unit(k), split);
       QuotientCols qc;
       uint64_t* e = (uint64_t*)ev.p;
       // columns `kept` moved to unit k, or `cnt` natural columns of `nat` evaluated on unit u into the next slots of ev
@@ -1052,6 +1174,84 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     for (uint32_t j = 0; j < T; j++) sources.push_back({table_cols[j], nullptr});
   }
   for (uint32_t i = 0; i < Q; i++) sources.push_back({qt_cols[2 * i], qt_cols[2 * i + 1]});
+  // compact and recompute plans: the natural-order columns behind the setup, witness and stage-2 oracles, in the order of
+  // the oracles' columns (so a row of them is the three oracles' leaves side by side), and the kept LDE column of each (on
+  // the recompute plan the oracles' columns are the natural ones themselves)
+  std::vector<const uint64_t*> nat;
+  std::unordered_map<const uint64_t*, uint32_t> nat_of;  // kept LDE column -> its index in nat
+  std::vector<char> pair_start;                          // nat[i], nat[i + 1] are the c0, c1 of one Fp2 polynomial
+  const uint32_t S = V + C + T;
+  if (compact || recompute) {
+    for (uint32_t j = 0; j < V; j++) nat.push_back(setup->sigmas + (size_t)j * n);
+    for (uint32_t j = 0; j < C; j++) nat.push_back(setup->constants + (size_t)j * n);
+    for (uint32_t j = 0; j < T; j++) nat.push_back(setup->tables + (size_t)j * n);
+    for (uint32_t j = 0; j < V; j++) nat.push_back(d_variables + (size_t)j * n);
+    if (lk) nat.push_back(d_multiplicities);
+    for (uint32_t j = 0; j < n_s2; j++) nat.push_back((const uint64_t*)st2.p + (size_t)j * n);
+    std::vector<const uint64_t*> kept(setup->tree.cols);
+    kept.insert(kept.end(), w_or.cols.begin(), w_or.cols.end());
+    kept.insert(kept.end(), s2_or.cols.begin(), s2_or.cols.end());
+    for (uint32_t i = 0; i < kept.size(); i++) nat_of[kept[i]] = i;
+    pair_start.assign(nat.size(), 0);
+    for (uint32_t j = 0; j < n_s2; j += 2) pair_start[S + w_or.cols.size() + j] = 1;
+  }
+  // chunks of `chunk` natural columns among nat[lo, hi) (an Fp2 pair never split): monomials by one iNTT, then body(c0, cnt,
+  // monomials, scratch for one coset of the chunk)
+  auto for_chunks = [&](uint32_t lo, uint32_t hi, const std::function<int32_t(uint32_t, uint32_t, const uint64_t*, uint64_t*)>& body) -> int32_t {
+    DevMem mono, ev;
+    BJ_TRY(mono.alloc(ctx, (size_t)chunk * n));
+    BJ_TRY(ev.alloc(ctx, (size_t)chunk * n));
+    for (uint32_t c0 = lo; c0 < hi;) {
+      uint32_t cnt = std::min<uint32_t>(chunk, hi - c0);
+      if (c0 + cnt < hi && pair_start[c0 + cnt - 1]) cnt--;
+      for (uint32_t i = 0; i < cnt; i++)
+        BJ_CUDA(ctx, cudaMemcpyAsync(mono.p + (size_t)i * n, nat[c0 + i], sizeof(u64) * n, cudaMemcpyDeviceToDevice, ctx->stream));
+      BJ_TRY(bj_intt_natural_to_natural(ctx, (uint64_t*)mono.p, log_n, cnt, n, 1));
+      BJ_TRY(body(c0, cnt, (const uint64_t*)mono.p, (uint64_t*)ev.p));
+      c0 += cnt;
+    }
+    return BJ_OK;
+  };
+  // recompute plan: the barycentric sums of the natural columns among flat from coset 0, rebuilt a chunk at a time (only the
+  // chunks that hold one of them), those of the quotient oracle's columns directly
+  auto open_rebuilt = [&](const std::vector<const uint64_t*>& flat, const uint64_t a[2], uint64_t* ev) -> int32_t {
+    auto evaluate = [&](const std::vector<const uint64_t*>& cols, const std::vector<size_t>& at) -> int32_t {
+      if (cols.empty()) return BJ_OK;
+      std::vector<uint64_t> got(2 * cols.size());
+      BJ_TRY(bj_barycentric_evaluate(ctx, cols.data(), (uint32_t)cols.size(), log_n, a, got.data()));
+      for (size_t k = 0; k < at.size(); k++) {
+        ev[2 * at[k]] = got[2 * k];
+        ev[2 * at[k] + 1] = got[2 * k + 1];
+      }
+      return BJ_OK;
+    };
+    std::vector<const uint64_t*> direct;
+    std::vector<size_t> direct_at;
+    uint32_t lo = (uint32_t)nat.size(), hi = 0;
+    for (size_t i = 0; i < flat.size(); i++) {
+      const auto it = nat_of.find(flat[i]);
+      if (it == nat_of.end()) {
+        direct.push_back(flat[i]);
+        direct_at.push_back(i);
+      } else {
+        lo = std::min(lo, it->second);
+        hi = std::max(hi, it->second + 1);
+      }
+    }
+    BJ_TRY(evaluate(direct, direct_at));
+    return for_chunks(lo, hi, [&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* on_coset) -> int32_t {
+      BJ_TRY(bj_lde_cosets(ctx, mono, n, on_coset, log_n, log_l, 0, 1, cnt, 1));
+      std::vector<const uint64_t*> cols;
+      std::vector<size_t> at;
+      for (size_t i = 0; i < flat.size(); i++) {
+        const auto it = nat_of.find(flat[i]);
+        if (it == nat_of.end() || it->second < c0 || it->second >= c0 + cnt) continue;
+        cols.push_back(on_coset + (size_t)(it->second - c0) * n);
+        at.push_back(i);
+      }
+      return evaluate(cols, at);
+    });
+  };
   auto open_at = [&](const std::vector<Src>& srcs, gl::e2 at, std::vector<gl::e2>& vals) -> int32_t {
     std::vector<const uint64_t*> flat;
     for (const auto& s : srcs) {
@@ -1062,7 +1262,9 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     if (flat.empty()) return BJ_OK;
     std::vector<uint64_t> ev(2 * flat.size());
     const uint64_t a[2] = {at.c0, at.c1};
-    if (world == 1) {
+    if (recompute) {
+      BJ_TRY(open_rebuilt(flat, a, ev.data()));
+    } else if (world == 1) {
       BJ_TRY(bj_barycentric_evaluate(ctx, flat.data(), (uint32_t)flat.size(), log_n, a, ev.data()));
     } else {
       // the columns are split over the coset groups: ranks [g B, (g + 1) B) hold the B row blocks of coset g (B = 1: one rank,
@@ -1139,43 +1341,6 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   DevMem deep;
   BJ_TRY(deep.alloc(ctx, 2 * nL));
   BJ_CUDA(ctx, cudaMemsetAsync(deep.p, 0, sizeof(u64) * 2 * nL, ctx->stream));
-  // compact plan: the natural-order columns behind the setup, witness and stage-2 oracles, in the order of the oracles'
-  // columns (so a row of them is the three oracles' leaves side by side), and the kept LDE column of each
-  std::vector<const uint64_t*> nat;
-  std::unordered_map<const uint64_t*, uint32_t> nat_of;  // kept LDE column -> its index in nat
-  std::vector<char> pair_start;                          // nat[i], nat[i + 1] are the c0, c1 of one Fp2 polynomial
-  const uint32_t S = V + C + T;
-  if (compact) {
-    for (uint32_t j = 0; j < V; j++) nat.push_back(setup->sigmas + (size_t)j * n);
-    for (uint32_t j = 0; j < C; j++) nat.push_back(setup->constants + (size_t)j * n);
-    for (uint32_t j = 0; j < T; j++) nat.push_back(setup->tables + (size_t)j * n);
-    for (uint32_t j = 0; j < V; j++) nat.push_back(d_variables + (size_t)j * n);
-    if (lk) nat.push_back(d_multiplicities);
-    for (uint32_t j = 0; j < n_s2; j++) nat.push_back((const uint64_t*)st2.p + (size_t)j * n);
-    std::vector<const uint64_t*> kept(setup->tree.cols);
-    kept.insert(kept.end(), w_or.cols.begin(), w_or.cols.end());
-    kept.insert(kept.end(), s2_or.cols.begin(), s2_or.cols.end());
-    for (uint32_t i = 0; i < kept.size(); i++) nat_of[kept[i]] = i;
-    pair_start.assign(nat.size(), 0);
-    for (uint32_t j = 0; j < n_s2; j += 2) pair_start[S + w_or.cols.size() + j] = 1;
-  }
-  // chunks of `chunk` natural columns (an Fp2 pair never split): monomials by one iNTT, then body(c0, cnt, monomials, scratch
-  // for one coset of the chunk)
-  auto for_chunks = [&](const std::function<int32_t(uint32_t, uint32_t, const uint64_t*, uint64_t*)>& body) -> int32_t {
-    DevMem mono, ev;
-    BJ_TRY(mono.alloc(ctx, (size_t)chunk * n));
-    BJ_TRY(ev.alloc(ctx, (size_t)chunk * n));
-    for (uint32_t c0 = 0; c0 < nat.size();) {
-      uint32_t cnt = std::min<uint32_t>(chunk, (uint32_t)nat.size() - c0);
-      if (c0 + cnt < nat.size() && pair_start[c0 + cnt - 1]) cnt--;
-      for (uint32_t i = 0; i < cnt; i++)
-        BJ_CUDA(ctx, cudaMemcpyAsync(mono.p + (size_t)i * n, nat[c0 + i], sizeof(u64) * n, cudaMemcpyDeviceToDevice, ctx->stream));
-      BJ_TRY(bj_intt_natural_to_natural(ctx, (uint64_t*)mono.p, log_n, cnt, n, 1));
-      BJ_TRY(body(c0, cnt, (const uint64_t*)mono.p, (uint64_t*)ev.p));
-      c0 += cnt;
-    }
-    return BJ_OK;
-  };
   struct DeepGroup {
     const std::vector<Src>* srcs;
     const std::vector<gl::e2>* vals;
@@ -1205,12 +1370,13 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   };
   auto deep_group = [&](const std::vector<Src>& srcs, const std::vector<gl::e2>& vals, gl::e2 at, const uint64_t* chs) -> int32_t {
     if (srcs.empty()) return BJ_OK;
-    if (compact) {
-      // cosets [0, Q) from the kept columns; the quotient oracle's columns hold all L cosets; the rest is recomputed below
+    if (compact || recompute) {
+      // cosets [0, first_rebuilt) from the kept columns; the quotient oracle's columns hold all L cosets; the rest is
+      // recomputed below
       const DeepGroup g{&srcs, &vals, at, chs};
       deep_groups.push_back(g);
-      BJ_TRY(deep_range(g, [](size_t) { return true; }, [](const uint64_t* p) { return p; }, 0, Qn));
-      return deep_range(g, [&](size_t i) { return !nat_of.count(srcs[i].c0); }, [&](const uint64_t* p) { return p + Qn; }, Qn, nL - Qn);
+      if (Fn) BJ_TRY(deep_range(g, [](size_t) { return true; }, [](const uint64_t* p) { return p; }, 0, Fn));
+      return deep_range(g, [&](size_t i) { return !nat_of.count(srcs[i].c0); }, [&](const uint64_t* p) { return p + Fn; }, Fn, nL - Fn);
     }
     std::vector<const uint64_t*> p0(srcs.size()), p1(srcs.size());
     std::vector<uint64_t> v(2 * srcs.size());
@@ -1234,14 +1400,14 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
       off += g.srcs.size();
     }
   }
-  if (compact)  // cosets [Q, L): every chunk of natural columns evaluated on one coset at a time, its DEEP terms added
-    BJ_TRY(for_chunks([&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* ev) -> int32_t {
+  if (compact || recompute)  // cosets [first_rebuilt, L): every chunk of natural columns evaluated on one coset at a time, its DEEP terms added
+    BJ_TRY(for_chunks(0, (uint32_t)nat.size(), [&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* ev) -> int32_t {
       auto in_chunk = [&](const uint64_t* p) {
         const auto it = nat_of.find(p);
         return it != nat_of.end() && it->second >= c0 && it->second < c0 + cnt;
       };
       auto on_coset = [&](const uint64_t* p) -> const uint64_t* { return ev + (size_t)(nat_of.at(p) - c0) * n; };
-      for (uint32_t j = Q; j < L; j++) {
+      for (uint32_t j = first_rebuilt; j < L; j++) {
         BJ_TRY(bj_lde_cosets(ctx, mono, n, ev, log_n, log_l, j, j + 1, cnt, 1));
         for (const DeepGroup& g : deep_groups)
           BJ_TRY(deep_range(g, [&](size_t i) { return in_chunk((*g.srcs)[i].c0); }, on_coset, (u64)j * n, n));
@@ -1307,7 +1473,9 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     while ((o->n_leaves >> depth) > o->cap_size) depth++;
     Part rows{std::vector<uint64_t>((size_t)num_queries * row_len), row_len};
     Part path{std::vector<uint64_t>((size_t)num_queries * depth * 4), (size_t)depth * 4};
-    if (compact && o != &qt_or) {  // kept columns hold cosets [0, Q); the rows of the other cosets are recomputed below
+    if (recompute && o != &qt_or) {
+      // no coset kept: every row is recomputed below
+    } else if (compact && o != &qt_or) {  // kept columns hold cosets [0, Q); the rows of the other cosets are recomputed below
       std::vector<uint64_t> kept_idx(loc_idx);
       for (auto& i : kept_idx)
         if (i >= Qn) i = 0;
@@ -1321,31 +1489,32 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     parts.push_back(std::move(rows));
     parts.push_back(std::move(path));
   }
-  if (compact) {
-    // queries whose leaf lies in a dropped coset j: one recompute of each such coset per chunk, the queried rows gathered
-    // from it.  Natural column i belongs to the setup (rows in parts[6]), witness (parts[0]) or stage-2 (parts[2]) oracle.
+  if (compact || recompute) {
+    // queries whose leaf lies in a coset j >= first_rebuilt: one recompute of each such coset per chunk, the queried rows
+    // gathered from it (the rows of every query, so that the gather buffer is the one the plan counts).  Natural column i
+    // belongs to the setup (rows in parts[6]), witness (parts[0]) or stage-2 (parts[2]) oracle.
     std::vector<std::vector<uint32_t>> by_coset(L);
     for (uint32_t q = 0; q < num_queries; q++)
-      if (idxs[q] >= Qn) by_coset[idxs[q] / n].push_back(q);
+      if (idxs[q] >= Fn) by_coset[idxs[q] / n].push_back(q);
     bool any = false;
-    for (uint32_t j = Q; j < L; j++) any = any || !by_coset[j].empty();
+    for (uint32_t j = first_rebuilt; j < L; j++) any = any || !by_coset[j].empty();
     const uint32_t Wc = (uint32_t)w_or.cols.size();
     if (any)
-      BJ_TRY(for_chunks([&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* ev) -> int32_t {
+      BJ_TRY(for_chunks(0, (uint32_t)nat.size(), [&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* ev) -> int32_t {
         std::vector<const uint64_t*> cols(cnt);
         for (uint32_t i = 0; i < cnt; i++) cols[i] = ev + (size_t)i * n;
-        for (uint32_t j = Q; j < L; j++) {
+        for (uint32_t j = first_rebuilt; j < L; j++) {
           const auto& qs = by_coset[j];
           if (qs.empty()) continue;
           BJ_TRY(bj_lde_cosets(ctx, mono, n, ev, log_n, log_l, j, j + 1, cnt, 1));
-          std::vector<uint64_t> rows_in(qs.size()), got(qs.size() * (size_t)cnt);
-          for (size_t k = 0; k < qs.size(); k++) rows_in[k] = idxs[qs[k]] - (u64)j * n;
-          BJ_TRY(bj_query_leaf_elements(ctx, cols.data(), cnt, 1, n, rows_in.data(), (uint32_t)qs.size(), got.data()));
+          std::vector<uint64_t> rows_in(num_queries, 0), got((size_t)num_queries * cnt);
+          for (uint32_t q : qs) rows_in[q] = idxs[q] - (u64)j * n;
+          BJ_TRY(bj_query_leaf_elements(ctx, cols.data(), cnt, 1, n, rows_in.data(), num_queries, got.data()));
           for (uint32_t i = 0; i < cnt; i++) {
             const uint32_t col = c0 + i;
             Part& pt = col < S ? parts[6] : col < S + Wc ? parts[0] : parts[2];
             const uint32_t within = col < S ? col : col < S + Wc ? col - S : col - S - Wc;
-            for (size_t k = 0; k < qs.size(); k++) pt.data[(size_t)qs[k] * pt.rec_len + within] = got[k * cnt + i];
+            for (uint32_t q : qs) pt.data[(size_t)q * pt.rec_len + within] = got[(size_t)q * cnt + i];
           }
         }
         return BJ_OK;
@@ -1496,18 +1665,26 @@ int32_t bj_proof_memory_plan_streamed_sharded(const bj_circuit* circuit, uint32_
   return BJ_OK;
 }
 
+int32_t bj_proof_memory_plan_recompute(const bj_circuit* circuit, uint32_t world, uint64_t* out) {
+  ProofShape sh;
+  if (!out) return BJ_ERR_INVALID_ARG;
+  BJ_TRY(memory_plan_shape(circuit, world, &sh));
+  *out = recompute_applies(sh) ? plan_bytes(sh, PLAN_RECOMPUTE) : 0;
+  return BJ_OK;
+}
+
 int32_t bj_setup_is_compact(const bj_setup* s) { return s ? (s->compact ? 1 : 0) : BJ_ERR_INVALID_ARG; }
 
 int32_t bj_setup_plan(const bj_setup* s) {
   if (!s) return BJ_ERR_INVALID_ARG;
-  return s->compact ? BJ_PLAN_COMPACT : s->streamed ? BJ_PLAN_STREAMED : BJ_PLAN_RESIDENT;
+  return s->compact ? BJ_PLAN_COMPACT : s->streamed ? BJ_PLAN_STREAMED : s->recompute ? BJ_PLAN_RECOMPUTE : BJ_PLAN_RESIDENT;
 }
 
 int32_t bj_setup_memory_plan(const bj_setup* s, uint64_t out[3]) {
   if (!s || !out) return BJ_ERR_INVALID_ARG;
   out[0] = s->pool_bytes;
   out[1] = s->outside_pool_bytes;
-  out[2] = s->compact ? s->chunk : 0;
+  out[2] = s->compact || s->recompute ? s->chunk : 0;
   return BJ_OK;
 }
 

@@ -50,6 +50,7 @@ SIGNATURES = {
     "bj_last_error": (ctypes.c_char_p, [_vp]),
     "bj_launch_count": (_u64, [_vp]),
     "bj_ctx_set_memory_limit": (_i32, [_vp, _u64]),
+    "bj_ctx_allow_recompute_plan": (_i32, [_vp, _i32]),
     "bj_ctx_memory_high_water": (_i32, [_vp, _vp, _i32]),
     "bj_alloc": (_i32, [_vp, _sz, _pp]),
     "bj_free": (_i32, [_vp, _vp]),
@@ -128,6 +129,7 @@ SIGNATURES = {
     "bj_proof_memory_plan": (_i32, [_vp, _u32, _vp]),
     "bj_proof_memory_plan_streamed": (_i32, [_vp, _u32, _vp]),
     "bj_proof_memory_plan_streamed_sharded": (_i32, [_vp, _u32, _vp]),
+    "bj_proof_memory_plan_recompute": (_i32, [_vp, _u32, _vp]),
     "bj_setup_is_compact": (_i32, [_vp]),
     "bj_setup_plan": (_i32, [_vp]),
     "bj_setup_memory_plan": (_i32, [_vp, _vp]),
@@ -187,7 +189,7 @@ class GateDesc(ctypes.Structure):
                 ("variables_initial_offset", ctypes.c_uint32), ("witnesses_initial_offset", ctypes.c_uint32)]
 
 
-PLAN_RESIDENT, PLAN_COMPACT, PLAN_STREAMED = range(3)  # BJ_PLAN_*
+PLAN_RESIDENT, PLAN_COMPACT, PLAN_STREAMED, PLAN_RECOMPUTE = range(4)  # BJ_PLAN_*
 IDX_VARIABLE, IDX_WITNESS, IDX_CONSTANT_POLY, IDX_TEMPORARY, IDX_CONSTANT_VALUE, IDX_CONSTANT_POLY_SHARED = range(6)
 REL_ADD, REL_DOUBLE, REL_SUB, REL_NEGATE, REL_MUL, REL_SQUARE, REL_INVERSE = range(7)
 

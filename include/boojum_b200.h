@@ -80,11 +80,17 @@ BJ_API uint64_t bj_launch_count(const bj_ctx* ctx);
 /* Device-memory limit of the prover driver on this context (bytes; 0, the default: what the device has free when
  * bj_setup_create runs, plus what the context's pool holds without using it).  bj_setup_create compares the memory plans of
  * bj_proof_memory_plan and bj_proof_memory_plan_streamed(_sharded) with it: RESIDENT if that fits, else COMPACT (one GPU,
- * quotient degree < LDE factor), else STREAMED (quotient degree > LDE factor, one GPU or sharded), else BJ_ERR_OOM with every
- * applicable byte count in the message and no kernel launched.  With quotient degree = LDE factor only RESIDENT applies.  On
+ * quotient degree < LDE factor), else STREAMED (quotient degree > LDE factor, one GPU or sharded), else RECOMPUTE (one GPU, only
+ * after bj_ctx_allow_recompute_plan(ctx, 1)), else BJ_ERR_OOM with every applicable byte count in the message and no kernel
+ * launched.  With quotient degree = LDE factor only RESIDENT (and the opt-in RECOMPUTE) applies.  On
  * a sharded context every rank chooses under its own limit; ranks on different plans still return the same proof.  bj_prove
  * follows the setup's plan and refuses the same way if the limit was lowered below it since. */
 BJ_API int32_t bj_ctx_set_memory_limit(bj_ctx* ctx, uint64_t bytes);
+/* allow != 0 lets bj_setup_create fall back to the RECOMPUTE plan (bj_proof_memory_plan_recompute) when none of RESIDENT,
+ * COMPACT and STREAMED fits under the limit; the refusal below every plan then names the recompute bytes too.  Off by default:
+ * the recompute plan rebuilds every coset of the setup, witness and stage-2 columns wherever it is read, so it is slower, and
+ * a caller that relies on BJ_ERR_OOM below the smaller plans keeps it.  A sharded context ignores the switch. */
+BJ_API int32_t bj_ctx_allow_recompute_plan(bj_ctx* ctx, int32_t allow);
 /* highest device memory the context's pool has had in use (cudaMemPoolAttrUsedMemHigh); reset != 0 restarts the mark.
  * Synchronises.  Memory the library keeps outside the pool (twiddles, coset-power tables, scratch) is not included. */
 BJ_API int32_t bj_ctx_memory_high_water(bj_ctx* ctx, uint64_t* bytes, int32_t reset);
@@ -511,16 +517,26 @@ BJ_API int32_t bj_proof_memory_plan_streamed(const bj_circuit* circuit, uint32_t
  * any other unit evaluated from the natural-order columns into one unit-sized scratch (with its z(omega x) columns on a
  * split shard).  The gathered quotient and everything after it are unchanged: every rank returns the single-GPU proof. */
 BJ_API int32_t bj_proof_memory_plan_streamed_sharded(const bj_circuit* circuit, uint32_t world, uint64_t* out);
-/* 1 if bj_setup_create chose the compact plan, 0 otherwise (resident or streamed) */
+/* The RECOMPUTE plan's bytes, counted the same way with 2 columns recomputed at a time (0 when world > 1).  It applies on one
+ * GPU to any quotient degree Q and LDE factor L, and keeps no coset of the setup, witness or stage-2 columns: only the trees,
+ * the natural-order stage-2 columns, the quotient oracle and the quotient buffers.  Each tree is built one committed coset at
+ * a time (the coset's columns evaluated from natural order into an n-row scratch per column, its n leaves hashed into their
+ * slice of the leaf array, the node levels after the last coset).  The quotient evaluates every column it reads onto one
+ * coset of [0, Q) at a time, the openings rebuild coset 0 a chunk of columns at a time, and DEEP and the query answers
+ * rebuild cosets [0, L) the same way.  Proofs are bit-identical to the resident plan's; opt in with
+ * bj_ctx_allow_recompute_plan. */
+BJ_API int32_t bj_proof_memory_plan_recompute(const bj_circuit* circuit, uint32_t world, uint64_t* out);
+/* 1 if bj_setup_create chose the compact plan, 0 otherwise (resident, streamed or recompute) */
 BJ_API int32_t bj_setup_is_compact(const bj_setup* setup);
-/* the plan bj_setup_create chose: BJ_PLAN_RESIDENT, BJ_PLAN_COMPACT or BJ_PLAN_STREAMED */
+/* the plan bj_setup_create chose: BJ_PLAN_RESIDENT, BJ_PLAN_COMPACT, BJ_PLAN_STREAMED or BJ_PLAN_RECOMPUTE */
 #define BJ_PLAN_RESIDENT 0
 #define BJ_PLAN_COMPACT 1
 #define BJ_PLAN_STREAMED 2
+#define BJ_PLAN_RECOMPUTE 3
 BJ_API int32_t bj_setup_plan(const bj_setup* setup);
 /* the plan bj_setup_create chose: out[0] the peak bytes of the context's pool over bj_setup_create + bj_prove (what
  * bj_ctx_memory_high_water reads on a fresh context), out[1] the bound on what the library holds outside the pool, out[2] the
- * columns the compact plan recomputes at a time (0 on the resident and streamed plans) */
+ * columns the compact or recompute plan recomputes at a time (0 on the resident and streamed plans) */
 BJ_API int32_t bj_setup_memory_plan(const bj_setup* setup, uint64_t out[3]);
 BJ_API int32_t bj_setup_get_cap(const bj_setup* setup, uint64_t* h_cap /* 4 * cap_size u64: VerificationKey::setup_merkle_tree_cap */);
 BJ_API int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables, const uint64_t* d_multiplicities /* or NULL */,
