@@ -678,3 +678,170 @@ API void orc_horner_ext(const uint64_t *mono, size_t n_cols, size_t n, const uin
     out[2 * c + 1] = acc.c1;
   }
 }
+
+/* ------------------------------------------------------------------------------------------------
+ * Gate programs: the recorded SSA programs (bj_gate_desc, include/boojum_b200.h) interpreted directly, one relation at a
+ * time, with canonical values - no peephole, no slot allocation, no step encoding - so these restate what
+ * bj_quotient_gates_general_purpose and the gate half of bj_check_satisfied compute independently of the compiler they run.
+ *   RowwiseEvaluator (repetitions, PerChunkOffset)     src/cs/traits/evaluator.rs:376-397
+ *   push_evaluation_result / proceed_to_next_gate      src/cs/implementations/buffering_source.rs:158-221, 304-362
+ *   compute_selector_subpath                           src/cs/implementations/prover.rs:2775-2916
+ *   check_if_satisfied (gates)                         src/cs/implementations/satisfiability_test.rs:15-353
+ * Flat arguments:
+ *   gates  [n_gates][ORC_GD_WORDS]: the descriptor fields below (path_bits: bit i = path[i]);
+ *   rels   [*][6]: op, dst temporary, a.kind, a.value, b.kind, b.value (BJ_REL_*, BJ_IDX_*), indexed from ORC_GD_REL_BEGIN;
+ *   writes [*][2]: kind, value, indexed from ORC_GD_WRITE_BEGIN;
+ *   cols: [variables | witnesses | constants], lazy u64 values.  The selector reads constant columns 0 .. path_len - 1.
+ * Inverse of 0 is 0.
+ * ---------------------------------------------------------------------------------------------- */
+enum {
+  ORC_GD_REL_BEGIN, ORC_GD_N_REL, ORC_GD_WRITE_BEGIN, ORC_GD_N_WRITES, ORC_GD_REPS, ORC_GD_VAR_OFF, ORC_GD_WIT_OFF,
+  ORC_GD_CONST_OFF, ORC_GD_CONST_PLACE, ORC_GD_PATH_LEN, ORC_GD_PATH_BITS, ORC_GD_VAR_INIT, ORC_GD_WIT_INIT, ORC_GD_WORDS
+};
+
+typedef struct {
+  const uint64_t *gates, *rels, *writes;
+  size_t n_gates;
+  const uint64_t *const *cols;
+  uint64_t n_vars, n_wits;
+  size_t n_tmp, max_writes; /* temporaries any program names, terms per repetition at most */
+} orc_gate_set;
+
+static orc_gate_set gate_set(const uint64_t *gates, size_t n_gates, const uint64_t *rels, const uint64_t *writes,
+                             const uint64_t *const *cols, uint32_t n_vars, uint32_t n_wits) {
+  orc_gate_set s = {gates, rels, writes, n_gates, cols, n_vars, n_wits, 1, 1};
+  for (size_t g = 0; g < n_gates; g++) {
+    const uint64_t *d = gates + g * ORC_GD_WORDS;
+    for (uint64_t i = 0; i < d[ORC_GD_N_REL]; i++)
+      if (rels[6 * (d[ORC_GD_REL_BEGIN] + i) + 1] + 1 > s.n_tmp) s.n_tmp = rels[6 * (d[ORC_GD_REL_BEGIN] + i) + 1] + 1;
+    if (d[ORC_GD_N_WRITES] > s.max_writes) s.max_writes = d[ORC_GD_N_WRITES];
+  }
+  return s;
+}
+
+static uint64_t gate_operand(const orc_gate_set *s, const uint64_t *d, uint64_t kind, uint64_t v, uint64_t rep, size_t t,
+                             const uint64_t *tmp) {
+  const uint64_t consts = s->n_vars + s->n_wits;
+  switch (kind) {
+    case 0: return gl_canon(s->cols[d[ORC_GD_VAR_INIT] + v + rep * d[ORC_GD_VAR_OFF]][t]);
+    case 1: return gl_canon(s->cols[s->n_vars + d[ORC_GD_WIT_INIT] + v + rep * d[ORC_GD_WIT_OFF]][t]);
+    case 2: return gl_canon(s->cols[consts + d[ORC_GD_CONST_PLACE] + v + rep * d[ORC_GD_CONST_OFF]][t]);
+    case 3: return tmp[v];
+    case 4: return gl_canon(v);
+    default: return gl_canon(s->cols[consts + d[ORC_GD_CONST_PLACE] + v][t]); /* row-shared constant: read at repetition 0 */
+  }
+}
+
+/* the terms of repetition `rep` of gate d at point t, in write order */
+static void gate_terms(const orc_gate_set *s, const uint64_t *d, uint64_t rep, size_t t, uint64_t *tmp, uint64_t *terms) {
+  for (uint64_t i = 0; i < d[ORC_GD_N_REL]; i++) {
+    const uint64_t *r = s->rels + 6 * (d[ORC_GD_REL_BEGIN] + i);
+    const uint64_t a = gate_operand(s, d, r[2], r[3], rep, t, tmp);
+    const int binary = r[0] == 0 || r[0] == 2 || r[0] == 4;
+    const uint64_t b = binary ? gate_operand(s, d, r[4], r[5], rep, t, tmp) : 0;
+    uint64_t v;
+    switch (r[0]) {
+      case 0: v = gl_add(a, b); break;
+      case 1: v = gl_dbl(a); break;
+      case 2: v = gl_sub(a, b); break;
+      case 3: v = gl_neg(a); break;
+      case 4: v = gl_mul(a, b); break;
+      case 5: v = gl_sqr(a); break;
+      default: v = gl_inv(a); break; /* 0 -> 0 */
+    }
+    tmp[r[1]] = v;
+  }
+  for (uint64_t k = 0; k < d[ORC_GD_N_WRITES]; k++) {
+    const uint64_t *w = s->writes + 2 * (d[ORC_GD_WRITE_BEGIN] + k);
+    terms[k] = gate_operand(s, d, w[0], w[1], rep, t, tmp);
+  }
+}
+
+static uint64_t gate_selector(const orc_gate_set *s, const uint64_t *d, size_t t) {
+  uint64_t sel = 1;
+  for (uint64_t i = 0; i < d[ORC_GD_PATH_LEN]; i++) {
+    const uint64_t c = gl_canon(s->cols[s->n_vars + s->n_wits + i][t]);
+    sel = gl_mul(sel, ((d[ORC_GD_PATH_BITS] >> i) & 1) ? c : gl_sub(1, c));
+  }
+  return sel;
+}
+
+/* q[t] += sum_g sel_g(t) * sum_k alpha[k] * term_k(t), k running on across gates and repetitions; alphas (c0, c1) per term */
+API void orc_gates_quotient(const uint64_t *gates, size_t n_gates, const uint64_t *rels, const uint64_t *writes,
+                            const uint64_t *const *cols, uint32_t n_vars, uint32_t n_wits, const uint64_t *alphas,
+                            size_t n_points, uint64_t *q0, uint64_t *q1) {
+  const orc_gate_set s = gate_set(gates, n_gates, rels, writes, cols, n_vars, n_wits);
+#pragma omp parallel
+  {
+    uint64_t *tmp = calloc(s.n_tmp, sizeof(uint64_t)), *terms = calloc(s.max_writes, sizeof(uint64_t));
+#pragma omp for schedule(static)
+    for (long tl = 0; tl < (long)n_points; tl++) {
+      const size_t t = (size_t)tl;
+      uint64_t r0 = gl_canon(q0[t]), r1 = gl_canon(q1[t]);
+      size_t k = 0;
+      for (size_t g = 0; g < n_gates; g++) {
+        const uint64_t *d = gates + g * ORC_GD_WORDS;
+        uint64_t a0 = 0, a1 = 0;
+        for (uint64_t rep = 0; rep < d[ORC_GD_REPS]; rep++) {
+          gate_terms(&s, d, rep, t, tmp, terms);
+          for (uint64_t j = 0; j < d[ORC_GD_N_WRITES]; j++, k++) {
+            a0 = gl_add(a0, gl_mul(terms[j], gl_canon(alphas[2 * k])));
+            a1 = gl_add(a1, gl_mul(terms[j], gl_canon(alphas[2 * k + 1])));
+          }
+        }
+        const uint64_t sel = gate_selector(&s, d, t);
+        r0 = gl_add(r0, gl_mul(sel, a0));
+        r1 = gl_add(r1, gl_mul(sel, a1));
+      }
+      q0[t] = r0;
+      q1[t] = r1;
+    }
+    free(tmp);
+    free(terms);
+  }
+}
+
+/* Check mode over n_rows rows: every term of every repetition of a gate must be 0 where the gate's selector is nonzero.
+ * out[0] = failing (row, gate, repetition) instances, out[1] = the first failing row, out[2] = its first failing global term
+ * index (term base of the gate + rep * n_writes + term) in (gate, repetition, term) order; first_value / first_selector [n_rows]
+ * = that term's value and its gate's selector on every failing row, 0 on the others.  out[1], out[2] are 0 without failures. */
+API void orc_gates_check(const uint64_t *gates, size_t n_gates, const uint64_t *rels, const uint64_t *writes,
+                         const uint64_t *const *cols, uint32_t n_vars, size_t n_rows, uint64_t *first_value,
+                         uint64_t *first_selector, uint64_t out[3]) {
+  const orc_gate_set s = gate_set(gates, n_gates, rels, writes, cols, n_vars, 0);
+  uint64_t failures = 0, first_key = UINT64_MAX;
+#pragma omp parallel reduction(+ : failures) reduction(min : first_key)
+  {
+    uint64_t *tmp = calloc(s.n_tmp, sizeof(uint64_t)), *terms = calloc(s.max_writes, sizeof(uint64_t));
+#pragma omp for schedule(static)
+    for (long tl = 0; tl < (long)n_rows; tl++) {
+      const size_t t = (size_t)tl;
+      uint64_t term_base = 0, row_term = UINT64_MAX;
+      first_value[t] = first_selector[t] = 0;
+      for (size_t g = 0; g < n_gates; g++) {
+        const uint64_t *d = gates + g * ORC_GD_WORDS;
+        const uint64_t sel = gate_selector(&s, d, t);
+        for (uint64_t rep = 0; sel && rep < d[ORC_GD_REPS]; rep++) {
+          gate_terms(&s, d, rep, t, tmp, terms);
+          for (uint64_t j = 0; j < d[ORC_GD_N_WRITES]; j++) {
+            if (!terms[j]) continue;
+            failures++;
+            if (row_term == UINT64_MAX) {
+              row_term = term_base + rep * d[ORC_GD_N_WRITES] + j;
+              first_value[t] = terms[j];
+              first_selector[t] = sel;
+            }
+            break;
+          }
+        }
+        term_base += d[ORC_GD_REPS] * d[ORC_GD_N_WRITES];
+      }
+      if (row_term != UINT64_MAX && (((uint64_t)t << 32) | row_term) < first_key) first_key = ((uint64_t)t << 32) | row_term;
+    }
+    free(tmp);
+    free(terms);
+  }
+  out[0] = failures;
+  out[1] = failures ? first_key >> 32 : 0;
+  out[2] = failures ? first_key & 0xffffffffu : 0;
+}

@@ -63,6 +63,8 @@ def lib():
             "orc_lookup_polys": (None, [vp, sz, sz, vp, vp, sz, vp, vp, vp, sz, vp]),
             "orc_lookup_quotient": (None, [vp, sz, sz, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp, sz, vp, vp]),
             "orc_horner_ext": (None, [vp, sz, sz, vp, vp]),
+            "orc_gates_quotient": (None, [vp, sz, vp, vp, vp, ctypes.c_uint32, ctypes.c_uint32, vp, sz, vp, vp]),
+            "orc_gates_check": (None, [vp, sz, vp, vp, vp, ctypes.c_uint32, sz, vp, vp, vp]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)
@@ -394,3 +396,71 @@ def random_field(rng, shape):
         a[bad] = rng.integers(0, 2**64, size=int(bad.sum()), dtype=np.uint64)
         bad = a >= np.uint64(P)
     return a
+
+
+# ------------------------------------------------------------------------------------------ gate programs -----
+_GD_WORDS = 13
+
+
+def _gate_arrays(gates):
+    """gate dicts (the form Context.evaluate_gates_over_general_purpose_columns takes) -> the flat descriptor, relation and
+    write arrays of orc_gates_quotient / orc_gates_check"""
+    desc, rels, writes = [], [], []
+    for g in gates:
+        path = g["selector_path"]
+        assert len(path) <= 32
+        desc.append([len(rels), len(g["relations"]), len(writes), len(g["writes"]), g["num_repetitions"], g.get("variables_offset", 0),
+                     g.get("witnesses_offset", 0), g.get("constants_offset", 0), g["constants_placement_offset"], len(path),
+                     sum(1 << i for i, bit in enumerate(path) if bit), g.get("variables_initial_offset", 0),
+                     g.get("witnesses_initial_offset", 0)])
+        for op, dst, a, b in g["relations"]:
+            b = b if b is not None else (4, 0)
+            rels.append([op, dst, a[0], int(a[1]), b[0], int(b[1])])
+        writes += [[k, int(v)] for k, v in g["writes"]]
+    return (_u64(np.array(desc, dtype=np.uint64).reshape(-1, _GD_WORDS)), _u64(np.array(rels, dtype=np.uint64).reshape(-1, 6)),
+            _u64(np.array(writes, dtype=np.uint64).reshape(-1, 2)))
+
+
+def gates_quotient(gates, variables, witnesses, constants, alphas, q0, q1):
+    """q + sum_g sel_g * sum_k alpha_k term_k at every point: what bj_quotient_gates_general_purpose computes, from the recorded
+    programs.  variables / witnesses / constants: lists of [n] columns or [cols, n] arrays (lazy u64); alphas: (c0, c1) per
+    term.  Returns canonical (q0, q1)."""
+    d, r, w = _gate_arrays(gates)
+    cols = list(variables) + list(witnesses) + list(constants)
+    pc, keep = _ptrs(cols)
+    al = _u64(np.array(alphas, dtype=np.uint64).reshape(-1))
+    o0, o1 = _u64(q0).copy(), _u64(q1).copy()
+    assert al.shape[0] >= 2 * sum(len(g["writes"]) * g["num_repetitions"] for g in gates)
+    assert all(c.shape[0] >= o0.shape[0] for c in keep)
+    lib().orc_gates_quotient(_p(d), len(gates), _p(r), _p(w), pc, len(variables), len(witnesses), _p(al), o0.shape[0], _p(o0), _p(o1))
+    return o0, o1
+
+
+def gates_check(gates, variables, constants):
+    """The gate half of bj_check_satisfied over the rows of the columns: dict(failures, row, term = first failing global term
+    index, first_value [n], first_selector [n] - the first failing term's value and its gate's selector per row, 0 on passing
+    rows)."""
+    d, r, w = _gate_arrays(gates)
+    pc, keep = _ptrs(list(variables) + list(constants))
+    n = keep[0].shape[0]
+    fv, fs, out = np.zeros(n, np.uint64), np.zeros(n, np.uint64), np.zeros(3, np.uint64)
+    lib().orc_gates_check(_p(d), len(gates), _p(r), _p(w), pc, len(variables), n, _p(fv), _p(fs), _p(out))
+    return dict(failures=int(out[0]), row=int(out[1]), term=int(out[2]), first_value=fv, first_selector=fs)
+
+
+def gates_report(gates, variables, constants):
+    """gates_check in the fields of bj_satisfiability_report: gate_failures, gate_row, gate_index, gate_repetition, gate_term,
+    gate_value, gate_selector (all 0 without failures)"""
+    c = gates_check(gates, variables, constants)
+    rep = dict(gate_failures=c["failures"], gate_row=0, gate_index=0, gate_repetition=0, gate_term=0, gate_value=0, gate_selector=0)
+    if c["failures"]:
+        t, base = c["term"], 0
+        for gi, g in enumerate(gates):
+            size = len(g["writes"]) * g["num_repetitions"]
+            if t < base + size:
+                break
+            base += size
+        row = c["row"]
+        rep.update(gate_row=row, gate_index=gi, gate_repetition=(t - base) // len(g["writes"]), gate_term=(t - base) % len(g["writes"]),
+                   gate_value=int(c["first_value"][row]), gate_selector=int(c["first_selector"][row]))
+    return rep
