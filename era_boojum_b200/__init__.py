@@ -223,6 +223,20 @@ class Context:
     def synchronize(self):
         self._check(lib.bj_ctx_synchronize(self._h))
 
+    def lane(self):
+        """bj_ctx_create_lane: a context on this one's device with its own stream and pool that proves against this
+        context's setups (NativeSetup.prove(..., ctx=lane)), concurrently with the other lanes from other threads.  It
+        inherits the memory limit and the recompute-plan switch; closing this context closes its lanes first."""
+        h = ctypes.c_void_p()
+        self._check(lib.bj_ctx_create_lane(self._h, ctypes.byref(h)))
+        import weakref
+        lane = Context.__new__(Context)
+        lane._torch, lane.device, lane._h, lane._stream = self._torch, self.device, h, None
+        lane._children = weakref.WeakSet()
+        lane.parent = self
+        self._children.add(lane)
+        return lane
+
     shard_rank, shard_world, shard_split = 0, 1, 0
 
     def set_coset_shard(self, rank, world, lde_degree):
@@ -711,6 +725,24 @@ def proof_memory_plan(log_n, num_variables, num_constants, quotient_degree, conf
             "streamed_sharded": int(sharded.value) or None, "recompute": int(recompute.value) or None}
 
 
+def proof_memory_plan_lanes(log_n, num_variables, num_constants, quotient_degree, config, plan, n_lanes, lookup=None):
+    """bj_proof_memory_plan_lanes_host: device bytes of one setup proved on n_lanes lanes at once on one GPU, on `plan`
+    ("resident", "compact", "streamed" or "recompute"), counted from the shapes (no device needed) -> dict(setup=bytes the
+    setup and the shared tables hold, lane=bytes each lane adds, total=setup + n_lanes * lane), or None where the plan does
+    not apply.  At one lane, total is proof_memory_plan()[plan]."""
+    c = native.Circuit()
+    c.log_n, c.num_variables, c.num_constants, c.quotient_degree = log_n, num_variables, num_constants, quotient_degree
+    c.fri_lde_factor, c.merkle_tree_cap_size = config.fri_lde_factor, config.merkle_tree_cap_size
+    c.security_level, c.pow_bits = config.security_level, config.pow_bits
+    if lookup:
+        c.lookup_width, c.lookup_num_repetitions = lookup["width"], lookup["num_repetitions"]
+    kind = {"resident": native.PLAN_RESIDENT, "compact": native.PLAN_COMPACT, "streamed": native.PLAN_STREAMED,
+            "recompute": native.PLAN_RECOMPUTE}[plan]
+    out = (ctypes.c_uint64 * 3)()
+    _ok(lib.bj_proof_memory_plan_lanes_host(ctypes.byref(c), kind, n_lanes, out), "bj_proof_memory_plan_lanes_host")
+    return {"setup": int(out[0]), "lane": int(out[1]), "total": int(out[2])} if out[2] else None
+
+
 def witness_slots_bytes(log_n, num_variables, n_slots, max_values=0, lookup=None, world=1):
     """bj_witness_slots_bytes: device bytes of a set of n_slots witness slots (with a WitnessVec buffer of max_values values and
     the u32 variables hint when max_values > 0) on each of `world` GPUs, counted from the shapes (no device needed)"""
@@ -875,12 +907,24 @@ class NativeSetup:
         from .prover import verification_key
         return verification_key(*self._vk_args, self.get_cap())
 
-    def prove(self, variables, multiplicities=None, timings=None, as_json=False):
-        """bj_prove -> the proof as a dict in the reference's serde shape (or the JSON text)."""
+    def prove(self, variables, multiplicities=None, timings=None, as_json=False, ctx=None):
+        """bj_prove -> the proof as a dict in the reference's serde shape (or the JSON text).  ctx: the setup's context (the
+        default) or one of its lanes (Context.lane)."""
+        ctx = ctx or self.ctx
         h = ctypes.c_void_p()
-        self.ctx._check(lib.bj_prove(self.ctx._h, self._h, self.ctx._ptr(variables),
-                                     self.ctx._ptr(multiplicities) if multiplicities is not None else None, ctypes.byref(h)))
+        ctx._check(lib.bj_prove(ctx._h, self._h, ctx._ptr(variables),
+                                ctx._ptr(multiplicities) if multiplicities is not None else None, ctypes.byref(h)))
         return self._proof_out(h, timings, as_json)
+
+    def memory_plan_lanes(self, n):
+        """bj_proof_memory_plan_lanes: the chosen plan split for n lanes proving at once -> dict(setup=bytes the setup and the
+        shared tables hold, lane=bytes each lane adds (its pool's high-water mark plus its scratch and parameter arena),
+        lane_pool=the pool part of lane, total=setup + n * lane)"""
+        out = (ctypes.c_uint64 * 3)()
+        _ok(lib.bj_proof_memory_plan_lanes(self._h, n, out), "bj_proof_memory_plan_lanes")
+        pool = ctypes.c_uint64()
+        _ok(lib.bj_proof_memory_plan_lane_pool(self._h, ctypes.byref(pool)), "bj_proof_memory_plan_lane_pool")
+        return {"setup": int(out[0]), "lane": int(out[1]), "total": int(out[2]), "lane_pool": int(pool.value)}
 
     def attach_variables_hint(self, hint):
         """bj_setup_attach_variables_hint: the DenseVariablesCopyHint [V, hint_rows] (reference `Variable`s, bit 63 =
@@ -928,6 +972,43 @@ class NativeSetup:
         finally:
             if own:
                 slots.close()
+
+    def prove_concurrent(self, witnesses, lanes=2, as_json=True):
+        """Proves several witnesses at once on this setup's GPU, yielding the proofs in input order (each the bytes
+        prove() returns).  witnesses: an iterable of (variables [V, n], multiplicities [n] or None) CUDA tensors, complete
+        on the current torch stream when they are taken from the iterable.  `lanes` lane contexts (Context.lane) prove
+        them from a thread pool, at most two witnesses per lane ahead of the one yielded; the lanes are closed at the end.
+        Lanes do not combine with witness slots or prove_stream: those run on the setup's own context."""
+        import collections
+        import queue
+        from concurrent.futures import ThreadPoolExecutor
+        torch = self.ctx._torch
+        ctxs = [self.ctx.lane() for _ in range(lanes)]
+        idle = queue.Queue()
+        for c in ctxs:
+            idle.put(c)
+
+        def one(w):
+            c = idle.get()
+            try:
+                return self.prove(w[0], w[1] if len(w) > 1 else None, as_json=as_json, ctx=c)
+            finally:
+                idle.put(c)
+
+        pool = ThreadPoolExecutor(max_workers=lanes)
+        try:
+            pending = collections.deque()
+            for w in witnesses:
+                torch.cuda.current_stream(self.ctx.device).synchronize()  # the lanes' streams do not wait for torch's
+                pending.append(pool.submit(one, w))
+                if len(pending) >= 2 * lanes:
+                    yield pending.popleft().result()
+            while pending:
+                yield pending.popleft().result()
+        finally:
+            pool.shutdown(wait=True, cancel_futures=True)
+            for c in ctxs:
+                c.close()
 
     def _proof_out(self, h, timings, as_json):
         """a bj_proof handle -> the proof as a dict or JSON text (the handle is freed)"""

@@ -202,8 +202,9 @@ extern "C" int32_t bj_pow_blake2s(bj_ctx* ctx, const uint8_t* h_seed, uint32_t s
   memcpy(words, h_seed, seed_len);
   void* d_seed;
   BJ_TRY(param_upload(ctx, words, sizeof(words), &d_seed));
-  unsigned long long* d_best = nullptr;
-  BJ_CUDA(ctx, cudaMalloc(&d_best, sizeof(unsigned long long)));
+  // one word per context, kept: a proof on a lane must not cudaMalloc / cudaFree (both synchronise the whole device)
+  if (!ctx->pow_best) BJ_CUDA(ctx, cudaMalloc(&ctx->pow_best, sizeof(unsigned long long)));
+  unsigned long long* d_best = ctx->pow_best;
   const unsigned long long none = ~0ull;
   const u64 batch = 1ull << 24;
   int32_t st = BJ_OK;
@@ -221,7 +222,6 @@ extern "C" int32_t bj_pow_blake2s(bj_ctx* ctx, const uint8_t* h_seed, uint32_t s
       st = BJ_ERR_CUDA;
     if (st != BJ_OK) break;
   }
-  cudaFree(d_best);
   if (st == BJ_ERR_CUDA) BJ_FAIL(ctx, BJ_ERR_CUDA, "bj_pow_blake2s: CUDA error");
   if (st != BJ_OK) BJ_FAIL(ctx, st, "bj_pow_blake2s: no solution found");
   *h_challenge = best;

@@ -1,6 +1,7 @@
 // Context management, device memory and host self-test hooks of the C-ABI (include/boojum_b200.h).
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include "ctx.hpp"
 
 namespace bj {
@@ -51,6 +52,66 @@ __global__ void field_selftest_kernel(u64 n, u64 seed, unsigned long long* misma
   if (gl::canon(gl::sub(a, gl::P)) != gl::canon(a)) bad++;
   if (gl::mul(a, b) >= gl::P) bad++;
   if (bad) atomicAdd(mismatches, (unsigned long long)bad);
+}
+}  // namespace bj
+
+namespace bj {
+// the prover driver allocates tens of GB per proof: a private pool that never trims keeps the second and later proofs free
+// of cudaMalloc / page-mapping cost (the default pool returns memory to the OS at every synchronisation); nullptr if the
+// device has none
+static cudaMemPool_t private_pool(int device) {
+  cudaMemPoolProps props = {};
+  props.allocType = cudaMemAllocationTypePinned;
+  props.handleTypes = cudaMemHandleTypeNone;
+  props.location.type = cudaMemLocationTypeDevice;
+  props.location.id = device;
+  cudaMemPool_t pool = nullptr;
+  if (cudaMemPoolCreate(&pool, &props) != cudaSuccess) {
+    cudaGetLastError();
+    return nullptr;
+  }
+  uint64_t keep = ~0ull;
+  cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+  return pool;
+}
+
+// a lane of `parent` (bj_ctx_create_lane checks the arguments and the memory first): the parent's device, settings and tunables,
+// its own non-blocking stream (no implicit ordering with the legacy default stream or with the other lanes) and pool, and
+// tw_* viewing the parent's twiddles.  Every table the parent queued before this call is complete when it returns.
+int32_t ctx_new_lane(bj_ctx* parent, bj_ctx** out) {
+  std::unique_ptr<bj_ctx> lane(new bj_ctx());
+  lane->device = parent->device;
+  lane->sm_count = parent->sm_count;
+  lane->l2_persist_bytes = parent->l2_persist_bytes;
+  lane->l2_window_max = parent->l2_window_max;
+  lane->ntt_use_v2 = parent->ntt_use_v2;
+  lane->ntt_max_tile_log = parent->ntt_max_tile_log;
+  lane->ntt_pass1_w = parent->ntt_pass1_w;
+  lane->ntt_chunk_mb = parent->ntt_chunk_mb;
+  lane->ntt_full_pow = parent->ntt_full_pow;
+  lane->gate_peephole = parent->gate_peephole;
+  lane->gate_points_per_thread = parent->gate_points_per_thread;
+  lane->ntt_l2_persist = 0;  // the carve-out is sized for one stream's table (ctx.hpp)
+  lane->ntt_bulk = parent->ntt_bulk;
+  lane->memory_limit = parent->memory_limit;
+  lane->allow_recompute_plan = parent->allow_recompute_plan;
+  lane->own_twiddles = false;
+  BJ_CUDA(parent, cudaStreamCreateWithFlags(&lane->stream, cudaStreamNonBlocking));
+  lane->own_stream = true;
+  lane->pool = private_pool(parent->device);
+  {
+    std::lock_guard<std::mutex> lock(parent->tables_mu);
+    const cudaError_t e = cudaStreamSynchronize(parent->stream);
+    if (e != cudaSuccess) {
+      cudaStreamDestroy(lane->stream);
+      if (lane->pool) cudaMemPoolDestroy(lane->pool);
+      BJ_FAIL(parent, BJ_ERR_CUDA, std::string("bj_ctx_create_lane: cudaStreamSynchronize: ") + cudaGetErrorString(e));
+    }
+    lane->parent = parent;
+    parent->lanes++;
+  }
+  *out = lane.release();
+  return BJ_OK;
 }
 }  // namespace bj
 
@@ -137,22 +198,7 @@ int32_t bj_ctx_create(int32_t device, void* stream, bj_ctx** out_ctx) {
   ctx->ntt_bulk = env_int("BJ_NTT_BULK", 0);
   ctx->ntt_l2_persist = env_int("BJ_NTT_L2_PERSIST", 1);
   ctx->ntt_chunk_mb = env_int("BJ_NTT_CHUNK_MB", 0);
-  {
-    // the prover driver allocates tens of GB per proof: a private pool that never trims keeps the second and later
-    // proofs free of cudaMalloc / page-mapping cost (the default pool returns memory to the OS at every synchronisation)
-    cudaMemPoolProps props = {};
-    props.allocType = cudaMemAllocationTypePinned;
-    props.handleTypes = cudaMemHandleTypeNone;
-    props.location.type = cudaMemLocationTypeDevice;
-    props.location.id = device;
-    if (cudaMemPoolCreate(&ctx->pool, &props) == cudaSuccess) {
-      uint64_t keep = ~0ull;
-      cudaMemPoolSetAttribute(ctx->pool, cudaMemPoolAttrReleaseThreshold, &keep);
-    } else {
-      cudaGetLastError();
-      ctx->pool = nullptr;
-    }
-  }
+  ctx->pool = private_pool(device);
   int32_t st = poseidon2_init_constants(ctx);
   if (st != BJ_OK) {
     if (ctx->pool) cudaMemPoolDestroy(ctx->pool);
@@ -166,18 +212,25 @@ int32_t bj_ctx_create(int32_t device, void* stream, bj_ctx** out_ctx) {
 int32_t bj_ctx_destroy(bj_ctx* ctx) {
   if (!ctx) return BJ_OK;
   bj::DeviceGuard device_guard(ctx);
+  if (const uint32_t alive = ctx->lanes.load())
+    BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_ctx_destroy: " + std::to_string(alive) + " lane(s) of this context are alive: destroy them first");
   cudaStreamSynchronize(ctx->stream);
   if (ctx->witness_stream) {  // uploads of witness slot sets still in flight finish before the memory goes
     cudaStreamSynchronize(ctx->witness_stream);
     cudaStreamDestroy(ctx->witness_stream);
   }
-  if (ctx->tw_fwd) cudaFree(ctx->tw_fwd);
-  if (ctx->tw_inv) cudaFree(ctx->tw_inv);
+  if (ctx->own_twiddles) {  // a lane's view of its parent's pair is not its own
+    if (ctx->tw_fwd) cudaFree(ctx->tw_fwd);
+    if (ctx->tw_inv) cudaFree(ctx->tw_inv);
+  }
   for (auto& e : ctx->pow_cache) {
     cudaFree(e.lo);
     cudaFree(e.hi);
     if (e.full) cudaFree(e.full);
   }
+  for (void* p : ctx->tables_retired) cudaFree(p);
+  if (ctx->pow_best) cudaFree(ctx->pow_best);
+  if (ctx->gate_program) cudaFree(ctx->gate_program);
   if (ctx->pool) cudaMemPoolDestroy(ctx->pool);
   if (ctx->scratch) cudaFree(ctx->scratch);
   if (ctx->ptr_table) cudaFree(ctx->ptr_table);
@@ -192,6 +245,11 @@ int32_t bj_ctx_destroy(bj_ctx* ctx) {
       cudaEventDestroy(ctx->ev_down[i]);
     }
   }
+  if (ctx->own_stream) cudaStreamDestroy(ctx->stream);
+  if (ctx->parent) {
+    std::lock_guard<std::mutex> lock(ctx->parent->tables_mu);
+    ctx->parent->lanes--;
+  }
   delete ctx;
   return BJ_OK;
 }
@@ -199,6 +257,7 @@ int32_t bj_ctx_destroy(bj_ctx* ctx) {
 int32_t bj_ctx_set_stream(bj_ctx* ctx, void* stream) {
   bj::DeviceGuard device_guard(ctx);
   if (!ctx) return BJ_ERR_INVALID_ARG;
+  if (ctx->parent) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_ctx_set_stream: a lane keeps the stream it was created with");
   BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   ctx->stream = (cudaStream_t)stream;
   return BJ_OK;

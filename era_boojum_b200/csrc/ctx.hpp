@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <algorithm>
+#include <atomic>
+#include <mutex>
 #include <string>
 #include <vector>
 #include "../../include/boojum_b200.h"
@@ -139,6 +141,33 @@ struct bj_ctx {
   uint32_t shard_log_lde = 0;  // LDE factor the shard was declared for (locates the coset bits of flat indices)
   uint64_t memory_limit = 0;   // bj_ctx_set_memory_limit: device bytes a proof may use (0: what is free when the setup is created)
   bool allow_recompute_plan = false;  // bj_ctx_allow_recompute_plan: bj_setup_create may fall back to the recompute plan (one GPU)
+  unsigned long long* pow_best = nullptr;  // bj_pow_blake2s's one-word result, allocated on first use
+  void* gate_program = nullptr;            // a long gate program's device copy (gates.cu), grown on demand, kept
+  size_t gate_program_bytes = 0;
+  // ---- lanes (bj_ctx_create_lane): contexts on the parent's device that prove against the parent's setups concurrently ----
+  // One rule per piece of state, so that distinct lanes of one parent may run bj_prove from different host threads at once:
+  //  - twiddles: the parent's.  A lane's tw_* view the parent's pair, read under the parent's tables_mu; a transform longer
+  //    than that pair makes the lane build a private pair (own_twiddles, freed with the lane).  A lane never grows the
+  //    parent's pair.  The parent grows its own pair under tables_mu and, while it has lanes, retires the replaced pair
+  //    (tables_retired, freed with the parent) instead of freeing it, so a lane's view stays valid.
+  //  - coset-power tables: the parent's pow_cache, shared.  Every lookup and insert, the parent's too, holds the parent's
+  //    tables_mu.  A missing table is built on the caller's stream and, when a lane could read it, that stream is
+  //    synchronised before the table is published, so a published table is complete.  While the parent has lanes its cache
+  //    is never flushed: the 64-entry flush retires the tables instead.  The 3 GiB budget of full tables is the parent's.
+  //  - scratch, parameter arena, long gate program buffer, pointer table, launch counter, kernel-attribute bookkeeping,
+  //    stream, pool, proof-of-work word and last_error: the lane's own, touched by the lane's thread only.  All of them
+  //    only grow, so after its first proof a lane allocates nothing outside its pool.
+  //  - the persisting-L2 window: the device's carve-out is sized for the one coset-power table of one stream, so lanes do
+  //    not pin (ntt_l2_persist = 0); N streams pinning N tables into one carve-out would only evict one another.
+  //  - Poseidon2 round constants: device constant memory written once by bj_ctx_create; a lane does not rewrite them.
+  //  - the setups of the parent are read only; bj_prove on a lane first waits for the setup's ready event.
+  // Teardown: bj_ctx_destroy refuses a context with lanes alive; lanes are destroyed first.
+  bj_ctx* parent = nullptr;       // a lane's parent (nullptr: a context of bj_ctx_create)
+  std::atomic<uint32_t> lanes{0};  // lanes of this context alive
+  std::mutex tables_mu;            // guards tw_*, pow_cache, pow_full_bytes, tables_retired and setups (see above)
+  std::vector<void*> tables_retired;
+  bool own_twiddles = true;        // false while a lane's tw_* view the parent's pair
+  std::vector<const bj_setup*> setups;  // setups alive on this context: bj_ctx_create_lane plans against them
 };
 
 #define BJ_FAIL(ctx, code, msg)          \

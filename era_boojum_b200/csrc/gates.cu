@@ -784,33 +784,35 @@ static int gate_points_per_thread(const bj_ctx* ctx, u64 n_points) {
   return n_points >= (u64)ctx->sm_count * 4 * 512 ? 4 : n_points >= (u64)ctx->sm_count * 4 * 256 ? 2 : 1;
 }
 
-struct GateProgramGuard {  // a long program's own buffer, freed (stream-ordered, i.e. after the kernel) on every exit path
-  void* p;
-  cudaStream_t s;
-  ~GateProgramGuard() {
-    if (p) cudaFreeAsync(p, s);
-  }
-};
-
 // gates, steps and the column table [variables | witnesses | constants] of a compiled program set -> p.gates, p.ops, p.cols,
-// p.consts_base.  Small programs ride in the parameter arena; a long one (the Poseidon2 flattened gate is ~9k relations) gets
-// its own stream-ordered buffer (*big_program: the caller's GateProgramGuard frees it, also when this fails)
+// p.consts_base.  Small programs ride in the parameter arena; a long one (the Poseidon2 flattened gate is ~9k relations) goes
+// to the context's program buffer, which only grows: repeated proofs allocate nothing here (a cudaMalloc / cudaFree would
+// synchronise the device and serialise the lanes of a context).  The copy is ordered on the stream after the last kernel
+// that read the previous program.
 static int32_t gate_program_upload(bj_ctx* ctx, const CompiledGates& compiled, std::vector<const u64*> table, uint32_t consts_base,
-                                   GateEvalParams* p, void** big_program) {
+                                   GateEvalParams* p) {
   const std::vector<PackedOp>& ops = compiled.ops;
   void* d;
   BJ_TRY(param_upload(ctx, compiled.gates.data(), sizeof(DevGate) * compiled.gates.size(), &d));
   p->gates = (const DevGate*)d;
   p->n_gates = (u32)compiled.gates.size();
   static const PackedOp dummy_op{};
-  *big_program = nullptr;
   const size_t ops_bytes = sizeof(PackedOp) * std::max<size_t>(ops.size(), 1);
   if (ops_bytes > (128u << 10)) {
-    BJ_CUDA(ctx, cudaMallocAsync(big_program, ops_bytes, ctx->stream));
-    const cudaError_t e = cudaMemcpyAsync(*big_program, ops.data(), ops_bytes, cudaMemcpyHostToDevice, ctx->stream);
+    if (ctx->gate_program_bytes < ops_bytes) {
+      if (ctx->gate_program) {
+        BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        BJ_CUDA(ctx, cudaFree(ctx->gate_program));
+        ctx->gate_program = nullptr;
+        ctx->gate_program_bytes = 0;
+      }
+      BJ_CUDA(ctx, cudaMalloc(&ctx->gate_program, ops_bytes));
+      ctx->gate_program_bytes = ops_bytes;
+    }
+    const cudaError_t e = cudaMemcpyAsync(ctx->gate_program, ops.data(), ops_bytes, cudaMemcpyHostToDevice, ctx->stream);
     if (e != cudaSuccess)
       BJ_FAIL(ctx, BJ_ERR_CUDA, std::string("gate program upload: ") + cudaGetErrorString(e));
-    d = *big_program;
+    d = ctx->gate_program;
   } else {
     BJ_TRY(param_upload(ctx, ops.empty() ? &dummy_op : ops.data(), ops_bytes, &d));
   }
@@ -864,7 +866,6 @@ extern "C" int32_t bj_quotient_gates_general_purpose(bj_ctx* ctx, const bj_gate_
   std::vector<u64> alphas(2 * (size_t)total_terms);
   for (size_t i = 0; i < alphas.size(); i++) alphas[i] = gl::canon(h_alpha_powers[i]);
   GateEvalParams p{};
-  GateProgramGuard program_guard{nullptr, ctx->stream};
   {
     std::vector<const u64*> table;
     table.reserve((size_t)n_variables + n_witnesses + n_constants + 1);
@@ -873,7 +874,7 @@ extern "C" int32_t bj_quotient_gates_general_purpose(bj_ctx* ctx, const bj_gate_
     for (uint32_t i = 0; i < n_constants; i++) table.push_back((const u64*)h_constant_cols[i]);
     for (const u64* c : table)
       if (!c) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_quotient_gates_general_purpose: NULL column");
-    BJ_TRY(gate_program_upload(ctx, compiled, table, n_variables + n_witnesses, &p, &program_guard.p));
+    BJ_TRY(gate_program_upload(ctx, compiled, table, n_variables + n_witnesses, &p));
   }
   void* d;
   static const u64 zero2[2] = {0, 0};

@@ -255,27 +255,68 @@ static PowSquares make_squares(u64 w) {
   return ps;
 }
 
+// a parent whose lanes are all gone frees the tables it retired while they lived.  Called on the parent's own thread under its
+// tables_mu, after its stream has drained: no lane is left to read them (bj_ctx_destroy synchronised each lane's stream) and
+// the parent's earlier kernels are done.  The full-table budget is then recounted from the cache.
+static int32_t release_retired(bj_ctx* owner) {
+  if (owner->tables_retired.empty() || owner->lanes.load() > 0) return BJ_OK;
+  BJ_CUDA(owner, cudaStreamSynchronize(owner->stream));
+  for (void* p : owner->tables_retired) cudaFree(p);
+  owner->tables_retired.clear();
+  owner->pow_full_bytes = 0;
+  for (const auto& e : owner->pow_cache)
+    if (e.full) owner->pow_full_bytes += sizeof(u64) << e.log_n;
+  return BJ_OK;
+}
+
 int32_t ensure_twiddles(bj_ctx* ctx, int log_n) {
   if (log_n < 1) log_n = 1;
   if (log_n > 32) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "log_n > 32 (two-adicity of the field)");
   if (ctx->tw_log >= log_n) return BJ_OK;
+  if (ctx->parent && !ctx->own_twiddles) {  // a lane: view the parent's pair if it is long enough (ctx.hpp)
+    bj_ctx* p = ctx->parent;
+    std::lock_guard<std::mutex> lock(p->tables_mu);
+    if (p->tw_log >= log_n) {
+      ctx->tw_fwd = p->tw_fwd;
+      ctx->tw_inv = p->tw_inv;
+      ctx->tw_log = p->tw_log;
+      return BJ_OK;
+    }
+    ctx->tw_fwd = ctx->tw_inv = nullptr;  // else a private pair below
+    ctx->tw_log = 0;
+    ctx->own_twiddles = true;
+  }
+  std::unique_lock<std::mutex> lock(ctx->tables_mu, std::defer_lock);
+  if (!ctx->parent) {  // lanes read the pair under this lock
+    lock.lock();
+    BJ_TRY(release_retired(ctx));
+  }
   // grow: tables of 2^(log_n-1) entries, tab[k] = w_{2^log_n}^{bitrev_{log_n-1}(k)} (prefix-stable)
   if (ctx->tw_fwd) {
     BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(ctx->tw_fwd);
-    cudaFree(ctx->tw_inv);
+    if (ctx->lanes.load() > 0) {  // a lane may still read the old pair
+      ctx->tables_retired.push_back(ctx->tw_fwd);
+      ctx->tables_retired.push_back(ctx->tw_inv);
+    } else {
+      cudaFree(ctx->tw_fwd);
+      cudaFree(ctx->tw_inv);
+    }
     ctx->tw_fwd = ctx->tw_inv = nullptr;
     ctx->tw_log = 0;
   }
   const u32 count = 1u << (log_n - 1);
-  BJ_CUDA(ctx, cudaMalloc(&ctx->tw_fwd, sizeof(u64) * count));
-  BJ_CUDA(ctx, cudaMalloc(&ctx->tw_inv, sizeof(u64) * count));
+  u64 *fwd = nullptr, *inv = nullptr;
+  BJ_CUDA(ctx, cudaMalloc(&fwd, sizeof(u64) * count));
+  BJ_CUDA(ctx, cudaMalloc(&inv, sizeof(u64) * count));
   const u64 w = gl::omega(log_n);
   const u32 blocks = (count + 255) / 256;
-  twiddle_table_kernel<<<blocks, 256, 0, ctx->stream>>>(ctx->tw_fwd, count, log_n - 1, make_squares(w));
+  twiddle_table_kernel<<<blocks, 256, 0, ctx->stream>>>(fwd, count, log_n - 1, make_squares(w));
   BJ_LAUNCH_CHECK(ctx);
-  twiddle_table_kernel<<<blocks, 256, 0, ctx->stream>>>(ctx->tw_inv, count, log_n - 1, make_squares(gl::inv(w)));
+  twiddle_table_kernel<<<blocks, 256, 0, ctx->stream>>>(inv, count, log_n - 1, make_squares(gl::inv(w)));
   BJ_LAUNCH_CHECK(ctx);
+  if (ctx->lanes.load() > 0) BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // complete before a lane can view it
+  ctx->tw_fwd = fwd;
+  ctx->tw_inv = inv;
   ctx->tw_log = log_n;
   return BJ_OK;
 }
@@ -294,20 +335,30 @@ __global__ void __launch_bounds__(256) pow_full_kernel(u64* __restrict__ full, u
 // (mostly L2-resident, shared by all columns) traffic are cheaper than 25 more instructions.
 static constexpr size_t POW_FULL_BUDGET = (size_t)3 << 30;
 static int32_t get_pow_tables(bj_ctx* ctx, u64 c, int log_n, u64 scale, PowTab* out) {
-  for (auto& e : ctx->pow_cache)
+  // a lane's tables are its parent's cache, built by whichever context misses first (ctx.hpp); the kernels run on ctx's stream
+  bj_ctx* owner = ctx->parent ? ctx->parent : ctx;
+  std::lock_guard<std::mutex> lock(owner->tables_mu);
+  if (owner == ctx) BJ_TRY(release_retired(ctx));
+  for (auto& e : owner->pow_cache)
     if (e.coset == c && e.log_n == log_n && e.scale == scale) {
       *out = e;
       return BJ_OK;
     }
-  if (ctx->pow_cache.size() >= 64) {  // bounded cache: drop everything (tables are cheap to rebuild)
+  const bool shared = owner->lanes.load() > 0;
+  if (owner->pow_cache.size() >= 64) {  // bounded cache: drop everything (tables are cheap to rebuild)
     BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    for (auto& e : ctx->pow_cache) {
+    for (auto& e : owner->pow_cache) {
+      if (shared) {  // a lane may still read them
+        owner->tables_retired.insert(owner->tables_retired.end(), {(void*)e.lo, (void*)e.hi});
+        if (e.full) owner->tables_retired.push_back(e.full);
+        continue;
+      }
       cudaFree(e.lo);
       cudaFree(e.hi);
       if (e.full) cudaFree(e.full);
     }
-    ctx->pow_cache.clear();
-    ctx->pow_full_bytes = 0;
+    owner->pow_cache.clear();
+    if (!shared) owner->pow_full_bytes = 0;  // retired full tables count against the budget until release_retired
   }
   PowTab pt;
   pt.coset = c;
@@ -325,17 +376,18 @@ static int32_t get_pow_tables(bj_ctx* ctx, u64 c, int log_n, u64 scale, PowTab* 
   BJ_LAUNCH_CHECK(ctx);
   pt.full = nullptr;
   const size_t full_bytes = sizeof(u64) << log_n;
-  if (ctx->ntt_full_pow && log_n >= 8 && ctx->pow_full_bytes + full_bytes <= POW_FULL_BUDGET &&
+  if (ctx->ntt_full_pow && log_n >= 8 && owner->pow_full_bytes + full_bytes <= POW_FULL_BUDGET &&
       cudaMalloc(&pt.full, full_bytes) == cudaSuccess) {
     const u64 n = 1ull << log_n;
     pow_full_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(pt.full, n, pt.lo, pt.hi, pt.split);
     BJ_LAUNCH_CHECK(ctx);
-    ctx->pow_full_bytes += full_bytes;
+    owner->pow_full_bytes += full_bytes;
   } else {
     cudaGetLastError();
     pt.full = nullptr;
   }
-  ctx->pow_cache.push_back(pt);
+  if (shared) BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // complete before another stream can read it
+  owner->pow_cache.push_back(pt);
   *out = pt;
   return BJ_OK;
 }

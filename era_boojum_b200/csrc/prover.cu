@@ -379,8 +379,9 @@ struct Ledger {
   void sub(u64 n_u64) { cur -= pool_bytes(n_u64); }
 };
 
-// peak pool bytes of bj_setup_create followed by bj_prove; `chunk`: columns recomputed at a time (compact and recompute plans)
-static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk) {
+// peak pool bytes of bj_setup_create followed by bj_prove; `chunk`: columns recomputed at a time (compact and recompute plans);
+// `setup_held`: the pool bytes the setup holds once bj_setup_create has returned
+static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk, u64* setup_held = nullptr) {
   Ledger m;
   const bool compact = plan == PLAN_COMPACT, streamed = plan == PLAN_STREAMED, recompute = plan == PLAN_RECOMPUTE;
   const u64 n = s.n, w = s.world, nL = (n << s.log_l) / w, nQ = n << s.log_q, Qn = n * s.Q;
@@ -424,6 +425,7 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk) {
     m.add(S * Qn);
     m.sub(S * nD);
   }
+  if (setup_held) *setup_held = m.cur;
   // the compact plan's column groups (lde_grouped / keep_first_cosets_grouped): sizes of the groups of n_cols columns
   auto groups = [](u32 n_cols) {
     std::vector<u64> g;
@@ -539,20 +541,32 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk) {
 // device bytes the library holds outside the pool during a proof (upper bounds): forward + inverse twiddles of the
 // factor-D domain, the coset-power tables (capped by their 3 GiB budget in ntt.cu), the NTT / LDE / opening scratch, and a
 // fixed 16 MiB for the parameter arena (8 MiB) and the long gate programs gates.cu uploads outside the context's pool
-static u64 library_reserve(const ProofShape& s) {
+// The first two are the tables a context's lanes share (library_tables), the last two each lane holds itself (lane_reserve).
+static u64 library_tables(const ProofShape& s) {
   const u64 n = s.n, D = 1ull << s.log_d;
-  u64 r = sizeof(u64) * n * D;
-  r += std::min<u64>(3ull << 30, sizeof(u64) * n * (D + s.Q + 2)) + 64 * 16 * (1ull << ((s.log_n + s.log_d + 2) / 2));
-  r += sizeof(u64) * std::max<u64>(1ull << 27, 4 * n);
-  r += 16ull << 20;
-  return r;
+  return sizeof(u64) * n * D + std::min<u64>(3ull << 30, sizeof(u64) * n * (D + s.Q + 2)) + 64 * 16 * (1ull << ((s.log_n + s.log_d + 2) / 2));
 }
+static u64 lane_reserve(const ProofShape& s) { return sizeof(u64) * std::max<u64>(1ull << 27, 4 * s.n) + (16ull << 20); }
+static u64 library_reserve(const ProofShape& s) { return library_tables(s) + lane_reserve(s); }
 
 static bool compact_applies(const ProofShape& s) { return s.world == 1 && s.Q < s.L; }
 static bool recompute_applies(const ProofShape& s) { return s.world == 1; }
 static bool streamed_applies(const ProofShape& s) { return s.Q > s.L; }  // on one GPU and on sharded contexts
 
 static u64 plan_bytes(const ProofShape& s, MemoryPlan plan, u32 chunk = 2) { return pool_peak(s, plan, chunk) + library_reserve(s); }
+
+// Lanes (bj_ctx_create_lane): one setup, proofs on n_lanes contexts at once.  The plan's bytes split in two: out[0] is the
+// setup's part (the pool bytes the setup holds after bj_setup_create, and the shared twiddle / coset-power tables), out[1] a
+// lane's part (the rest of the plan's pool peak, which is what a proof adds on top of the setup, and the lane's own scratch
+// and parameter arena), out[2] = out[0] + n_lanes * out[1].  At one lane out[0] + out[1] is the plan.  The lane's pool part is
+// its pool's high-water mark, or, where bj_setup_create itself peaks higher, that peak above what the setup keeps.
+static void lane_plan(const ProofShape& s, MemoryPlan plan, u32 chunk, u32 n_lanes, uint64_t out[3]) {
+  u64 held = 0;
+  const u64 peak = pool_peak(s, plan, chunk, &held);
+  out[0] = held + library_tables(s);
+  out[1] = (peak - held) + lane_reserve(s);
+  out[2] = out[0] + (u64)n_lanes * out[1];
+}
 
 }  // namespace bj
 
@@ -580,6 +594,7 @@ struct bj_setup {
   uint64_t hint_rows = 0;
   uint64_t hint_values = 0;  // 1 + the largest index the hint names: an all_values vector needs at least this many values
   bool has_hint = false;
+  cudaEvent_t ready = nullptr;  // recorded on the context's stream when bj_setup_create returns: bj_prove on a lane waits for it
   const uint64_t* col(uint32_t j) const { return (const uint64_t*)lde.p + (size_t)j * col_len; }
   uint32_t log_l() const {
     uint32_t l = 0;
@@ -612,6 +627,10 @@ struct bj_proof {
 };
 
 using namespace bj;
+
+namespace bj {
+int32_t ctx_new_lane(bj_ctx* parent, bj_ctx** out);  // capi.cu
+}
 
 static bool is_pow2(uint32_t x) { return x && !(x & (x - 1)); }
 
@@ -655,6 +674,8 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
                                 circuit->lookup_variables_offset + circuit->lookup_width * circuit->lookup_num_repetitions >
                                     circuit->num_variables))
     BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_setup_create: inconsistent lookup description");
+  if (ctx->parent)
+    BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_setup_create: a lane proves against its parent's setups: create the setup on the parent");
   if (ctx->shard.log_stride && !ctx->comm)
     BJ_FAIL(ctx, BJ_ERR_UNSUPPORTED, "bj_setup_create: a coset-sharded context needs a communicator (bj_comm_create_*) for the native driver");
   const uint32_t split = ctx->shard.log_split;  // row blocks per coset = 2^split when there are more ranks than cosets
@@ -684,6 +705,17 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
     }
   }
   std::unique_ptr<bj_setup> s(new bj_setup());
+  // the setup is handed out with an event recorded behind its last kernel (lanes wait for it) and is listed on the context
+  auto publish = [&]() -> int32_t {
+    BJ_CUDA(ctx, cudaEventCreateWithFlags(&s->ready, cudaEventDisableTiming));
+    BJ_CUDA(ctx, cudaEventRecord(s->ready, ctx->stream));
+    {
+      std::lock_guard<std::mutex> lock(ctx->tables_mu);
+      ctx->setups.push_back(s.get());
+    }
+    *out = s.release();
+    return BJ_OK;
+  };
   {
     // the memory plan: resident if it fits under the limit, else compact (Q < L, one GPU), else streamed (Q > L), else
     // recompute (one GPU, when the context allows it); refused before anything is launched.  On a sharded context every
@@ -696,12 +728,25 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
     s->plan[2] = streamed_applies(sh) ? plan_bytes(sh, PLAN_STREAMED) : 0;
     s->plan[3] = ctx->allow_recompute_plan && recompute_applies(sh) ? plan_bytes(sh, PLAN_RECOMPUTE) : 0;
     BJ_TRY(memory_limit(ctx, &s->limit));
-    auto fits = [&](int k) { return s->plan[k] && s->plan[k] <= s->limit; };
-    if (s->plan[0] > s->limit) {
+    // with lanes alive on the context, a plan must also hold their proofs: one lane part each beside the plan
+    const uint32_t lanes = ctx->lanes.load();
+    uint64_t need[4];
+    for (int k = 0; k < 4; k++) {
+      need[k] = s->plan[k];
+      if (need[k] && lanes) {
+        uint64_t lp[3];
+        lane_plan(sh, (MemoryPlan)k, 2, 1, lp);
+        need[k] += (uint64_t)lanes * lp[1];
+      }
+    }
+    auto fits = [&](int k) { return need[k] && need[k] <= s->limit; };
+    if (need[0] > s->limit) {
       if (fits(2)) s->streamed = true;
       else if (fits(1)) s->compact = true;
       else if (fits(3)) s->recompute = true;
-      else BJ_FAIL(ctx, BJ_ERR_OOM, plan_message("bj_setup_create", s->plan, s->limit));
+      else
+        BJ_FAIL(ctx, BJ_ERR_OOM, plan_message("bj_setup_create", need, s->limit) +
+                                     (lanes ? " (each plan counted with the " + std::to_string(lanes) + " lane(s) of the context)" : std::string()));
     }
     if (s->compact || s->recompute) {
       // wider recompute chunks only save kernel launches: the chunk grows into at most half of the headroom the limit leaves
@@ -761,8 +806,7 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
   if (s->recompute) {
     BJ_TRY(oracle_build_by_coset(ctx, s->tree, {{d_sigmas, V}, {d_constants, C}, {d_lookup_tables, T}}, log_n, log_l,
                                  circuit->merkle_tree_cap_size, circuit->tree_hasher));
-    *out = s.release();
-    return BJ_OK;
+    return publish();
   }
   const uint32_t log_kept = s->streamed ? log_l : log_d;
   s->col_len = (n << log_kept) / comm_world(ctx);
@@ -778,14 +822,19 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
     std::swap(s->lde.p, kept.p);
     s->col_len = n * circuit->quotient_degree;
   }
-  *out = s.release();
-  return BJ_OK;
+  return publish();
 }
 
 void bj_setup_free(bj_setup* s) {
   if (!s) return;
   bj::DeviceGuard device_guard(s->ctx);
-  if (s->ctx) cudaStreamSynchronize(s->ctx->stream);
+  if (s->ctx) {
+    cudaStreamSynchronize(s->ctx->stream);
+    std::lock_guard<std::mutex> lock(s->ctx->tables_mu);
+    auto& v = s->ctx->setups;
+    v.erase(std::remove(v.begin(), v.end(), s), v.end());
+  }
+  if (s->ready) cudaEventDestroy(s->ready);
   delete s;
 }
 
@@ -797,7 +846,10 @@ int32_t bj_setup_get_cap(const bj_setup* s, uint64_t* h_cap) {
 
 int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables, const uint64_t* d_multiplicities, bj_proof** out) {
   bj::DeviceGuard device_guard(ctx);
-  if (!ctx || !setup || !d_variables || !out || setup->ctx != ctx) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: bad argument");
+  // a lane proves against its parent's setups
+  if (!ctx || !setup || !d_variables || !out || (setup->ctx != ctx && (!ctx->parent || setup->ctx != ctx->parent)))
+    BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: bad argument");
+  if (setup->ctx != ctx) BJ_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, setup->ready, 0));
   const bj_circuit& c = setup->c;
   const bool lk = c.lookup_width != 0;
   if (lk && !d_multiplicities) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: the lookup argument needs the multiplicities column");
@@ -1671,6 +1723,70 @@ int32_t bj_proof_memory_plan_recompute(const bj_circuit* circuit, uint32_t world
   BJ_TRY(memory_plan_shape(circuit, world, &sh));
   *out = recompute_applies(sh) ? plan_bytes(sh, PLAN_RECOMPUTE) : 0;
   return BJ_OK;
+}
+
+int32_t bj_proof_memory_plan_lanes_host(const bj_circuit* circuit, uint32_t plan, uint32_t n_lanes, uint64_t out[3]) {
+  ProofShape sh;
+  if (!out || n_lanes == 0 || plan > BJ_PLAN_RECOMPUTE) return BJ_ERR_INVALID_ARG;
+  BJ_TRY(memory_plan_shape(circuit, 1, &sh));
+  const bool applies = plan == PLAN_RESIDENT || (plan == PLAN_COMPACT && compact_applies(sh)) || (plan == PLAN_STREAMED && streamed_applies(sh)) ||
+                       (plan == PLAN_RECOMPUTE && recompute_applies(sh));
+  if (!applies) {
+    out[0] = out[1] = out[2] = 0;
+    return BJ_OK;
+  }
+  lane_plan(sh, (MemoryPlan)plan, 2, n_lanes, out);
+  return BJ_OK;
+}
+
+static MemoryPlan setup_plan_kind(const bj_setup* s) {
+  return s->compact ? PLAN_COMPACT : s->streamed ? PLAN_STREAMED : s->recompute ? PLAN_RECOMPUTE : PLAN_RESIDENT;
+}
+
+int32_t bj_proof_memory_plan_lanes(const bj_setup* setup, uint32_t n_lanes, uint64_t out[3]) {
+  ProofShape sh;
+  if (!setup || !out || n_lanes == 0 || comm_world(setup->ctx) != 1) return BJ_ERR_INVALID_ARG;
+  BJ_TRY(proof_shape(setup->c, 1, &sh));
+  lane_plan(sh, setup_plan_kind(setup), setup->chunk, n_lanes, out);
+  return BJ_OK;
+}
+
+int32_t bj_proof_memory_plan_lane_pool(const bj_setup* setup, uint64_t* pool_bytes) {
+  ProofShape sh;
+  if (!setup || !pool_bytes || comm_world(setup->ctx) != 1) return BJ_ERR_INVALID_ARG;
+  BJ_TRY(proof_shape(setup->c, 1, &sh));
+  uint64_t out[3];
+  lane_plan(sh, setup_plan_kind(setup), setup->chunk, 1, out);
+  *pool_bytes = out[1] - lane_reserve(sh);
+  return BJ_OK;
+}
+
+int32_t bj_ctx_create_lane(bj_ctx* parent, bj_ctx** out) {
+  if (!out) BJ_FAIL(parent, BJ_ERR_INVALID_ARG, "bj_ctx_create_lane: out is NULL");
+  *out = nullptr;
+  if (!parent) return BJ_ERR_INVALID_ARG;
+  bj::DeviceGuard device_guard(parent);
+  if (parent->parent) BJ_FAIL(parent, BJ_ERR_INVALID_ARG, "bj_ctx_create_lane: a lane has no lanes of its own: create them on its parent");
+  if (parent->comm || parent->shard.log_stride)
+    BJ_FAIL(parent, BJ_ERR_INVALID_ARG, "bj_ctx_create_lane: a sharded context (communicator or domain shard) has no lanes");
+  {
+    // every setup of the parent, with the lanes alive, this one, and the parent itself (its pool keeps what its setup and its
+    // own proofs reached, so it counts as one proving context) must fit under the limit its plan was chosen under
+    std::lock_guard<std::mutex> lock(parent->tables_mu);
+    const uint32_t lanes_after = parent->lanes.load() + 1;
+    for (const bj_setup* s : parent->setups) {
+      ProofShape sh;
+      BJ_TRY(proof_shape(s->c, 1, &sh));
+      uint64_t p[3];
+      lane_plan(sh, setup_plan_kind(s), s->chunk, lanes_after + 1, p);
+      const uint64_t limit = parent->memory_limit ? parent->memory_limit : s->limit;
+      if (p[2] > limit)
+        BJ_FAIL(parent, BJ_ERR_OOM, "bj_ctx_create_lane: the setup's plan needs " + std::to_string(s->chosen_bytes()) + " bytes and every lane " +
+                                        std::to_string(p[1]) + " bytes more; with " + std::to_string(lanes_after) + " lane(s) that is " +
+                                        std::to_string(p[2]) + " bytes, above the limit of " + std::to_string(limit) + " bytes");
+    }
+  }
+  return ctx_new_lane(parent, out);
 }
 
 int32_t bj_setup_is_compact(const bj_setup* s) { return s ? (s->compact ? 1 : 0) : BJ_ERR_INVALID_ARG; }

@@ -431,11 +431,10 @@ extern "C" int32_t bj_check_satisfied(bj_ctx* ctx, const bj_circuit* circuit, co
   if (c.n_gates) {
     BJ_TRY(gate_first.alloc(ctx, 2 * n));
     GateEvalParams p{};
-    GateProgramGuard program_guard{nullptr, ctx->stream};
     std::vector<const u64*> table;
     for (u32 j = 0; j < V; j++) table.push_back((const u64*)d_variables + (size_t)j * n);
     for (u32 j = 0; j < c.num_constants; j++) table.push_back((const u64*)d_constants + (size_t)j * n);
-    BJ_TRY(gate_program_upload(ctx, compiled, table, V, &p, &program_guard.p));
+    BJ_TRY(gate_program_upload(ctx, compiled, table, V, &p));
     p.n_rows = n;
     GateCheckOut chk{gate_first.p, gate_first.p + n, &d_acc->gate_failures, &d_acc->gate_key};
     const int k_pts = gate_points_per_thread(ctx, n);

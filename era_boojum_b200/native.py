@@ -52,6 +52,7 @@ SIGNATURES = {
     "bj_ctx_set_memory_limit": (_i32, [_vp, _u64]),
     "bj_ctx_allow_recompute_plan": (_i32, [_vp, _i32]),
     "bj_ctx_memory_high_water": (_i32, [_vp, _vp, _i32]),
+    "bj_ctx_create_lane": (_i32, [_vp, _pp]),
     "bj_alloc": (_i32, [_vp, _sz, _pp]),
     "bj_free": (_i32, [_vp, _vp]),
     "bj_upload": (_i32, [_vp, _vp, _vp, _sz]),
@@ -133,6 +134,9 @@ SIGNATURES = {
     "bj_setup_is_compact": (_i32, [_vp]),
     "bj_setup_plan": (_i32, [_vp]),
     "bj_setup_memory_plan": (_i32, [_vp, _vp]),
+    "bj_proof_memory_plan_lanes": (_i32, [_vp, _u32, _vp]),
+    "bj_proof_memory_plan_lane_pool": (_i32, [_vp, _vp]),
+    "bj_proof_memory_plan_lanes_host": (_i32, [_vp, _u32, _u32, _vp]),
     "bj_setup_get_cap": (_i32, [_vp, _vp]),
     "bj_prove": (_i32, [_vp, _vp, _vp, _vp, _pp]),
     "bj_proof_free": (None, [_vp]),

@@ -94,6 +94,21 @@ BJ_API int32_t bj_ctx_allow_recompute_plan(bj_ctx* ctx, int32_t allow);
 /* highest device memory the context's pool has had in use (cudaMemPoolAttrUsedMemHigh); reset != 0 restarts the mark.
  * Synchronises.  Memory the library keeps outside the pool (twiddles, coset-power tables, scratch) is not included. */
 BJ_API int32_t bj_ctx_memory_high_water(bj_ctx* ctx, uint64_t* bytes, int32_t reset);
+/* Lanes: several proofs of one setup in flight on one GPU.  A lane is a context on the parent's device with its own stream
+ * (non-blocking), stream-ordered pool, scratch, parameter arena, launch counter and last error; it inherits the parent's memory
+ * limit and recompute-plan switch.  bj_prove(lane, setup, ...) takes a setup created on the parent and returns the bytes
+ * bj_prove(parent, setup, ...) returns, on every single-GPU plan.  Distinct lanes of one parent may run bj_prove at the same
+ * time from different host threads (one thread per lane); they read the setup and the parent's twiddle and coset-power tables,
+ * which nothing frees while a lane is alive.  After its first proof a lane allocates every proof buffer from its pool (no
+ * cudaMalloc / cudaFree).  A lane creates no setup, has no lanes and keeps its stream (bj_ctx_set_stream is refused).
+ * Refused with BJ_ERR_INVALID_ARG on a sharded parent (communicator or domain shard) and with BJ_ERR_OOM, naming the bytes and
+ * the limit and launching nothing, when for some setup alive on the parent bj_proof_memory_plan_lanes(setup, lanes + 1)[2]
+ * exceeds the parent's limit (bj_ctx_set_memory_limit, else the one the setup was planned under): `lanes` counts the lanes
+ * alive after this one, and the parent counts as one more because its pool keeps what its setup and its own proofs reached.
+ * A bj_setup_create on a parent with lanes alive counts them too: each plan must fit with one lane part per live lane.
+ * Create the lanes of one parent from one thread.  Teardown: bj_ctx_destroy(parent) refuses with BJ_ERR_INVALID_ARG while a
+ * lane is alive (destroy the lanes first); a setup may be freed once every bj_prove that reads it has returned. */
+BJ_API int32_t bj_ctx_create_lane(bj_ctx* parent, bj_ctx** out_lane);
 
 /* ---- multi-GPU: communicator of the sharded prover (one process - or one thread - per GPU) ----
  * Creating a communicator on a context declares its domain shard (bj_ctx_set_domain_shard(ctx, rank, world, log_lde)) and makes
@@ -538,6 +553,19 @@ BJ_API int32_t bj_setup_plan(const bj_setup* setup);
  * bj_ctx_memory_high_water reads on a fresh context), out[1] the bound on what the library holds outside the pool, out[2] the
  * columns the compact or recompute plan recomputes at a time (0 on the resident and streamed plans) */
 BJ_API int32_t bj_setup_memory_plan(const bj_setup* setup, uint64_t out[3]);
+/* device bytes of one setup proved on n_lanes >= 1 lanes at once (bj_ctx_create_lane), the setup's chosen plan split in two:
+ * out[0] the setup's part (the pool bytes it holds after bj_setup_create, and the twiddle and coset-power tables the lanes
+ * share), out[1] one lane's part (what a proof's pool adds on top of the setup - a fresh lane's bj_ctx_memory_high_water - and
+ * the lane's own scratch and parameter arena), out[2] = out[0] + n_lanes * out[1].  With n_lanes = 1, out[2] is the plan
+ * (bj_setup_memory_plan out[0] + out[1]).  BJ_ERR_INVALID_ARG for a setup of a sharded context. */
+BJ_API int32_t bj_proof_memory_plan_lanes(const bj_setup* setup, uint32_t n_lanes, uint64_t out[3]);
+/* the pool part of bj_proof_memory_plan_lanes out[1]: what a fresh lane's bj_ctx_memory_high_water reaches proving the setup
+ * (the rest of out[1] is the lane's scratch and parameter arena) */
+BJ_API int32_t bj_proof_memory_plan_lane_pool(const bj_setup* setup, uint64_t* pool_bytes);
+/* the same from the circuit's shapes alone (no device), for plan = BJ_PLAN_RESIDENT / COMPACT / STREAMED / RECOMPUTE on one GPU
+ * with the smallest recompute chunk: out[0] + out[1] equals bj_proof_memory_plan(_streamed / _recompute) for that plan; all
+ * three are 0 where the plan does not apply to the circuit */
+BJ_API int32_t bj_proof_memory_plan_lanes_host(const bj_circuit* circuit, uint32_t plan, uint32_t n_lanes, uint64_t out[3]);
 BJ_API int32_t bj_setup_get_cap(const bj_setup* setup, uint64_t* h_cap /* 4 * cap_size u64: VerificationKey::setup_merkle_tree_cap */);
 BJ_API int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables, const uint64_t* d_multiplicities /* or NULL */,
                  bj_proof** out);
