@@ -268,6 +268,12 @@ class Context:
         other plan fits under the limit.  Off by default; a sharded context ignores it."""
         self._check(lib.bj_ctx_allow_recompute_plan(self._h, int(bool(allow))))
 
+    def allow_sharded_recompute_plan(self, allow=True):
+        """bj_ctx_allow_sharded_recompute_plan: with allow, native_setup on a context with a communicator falls back to the
+        recompute plan on this rank (proof_memory_plan_recompute_sharded) when neither the resident nor the streamed plan fits
+        under the rank's limit.  Off by default; a context without a communicator ignores it."""
+        self._check(lib.bj_ctx_allow_sharded_recompute_plan(self._h, int(bool(allow))))
+
     def memory_high_water(self, reset=False):
         """bj_ctx_memory_high_water: the highest device memory the context's pool has had in use (bytes)"""
         v = ctypes.c_uint64()
@@ -723,6 +729,22 @@ def proof_memory_plan(log_n, num_variables, num_constants, quotient_degree, conf
     _ok(lib.bj_proof_memory_plan_recompute(ctypes.byref(c), world, ctypes.byref(recompute)), "bj_proof_memory_plan_recompute")
     return {"resident": int(out[0]), "compact": int(out[1]) or None, "streamed": int(streamed.value) or None,
             "streamed_sharded": int(sharded.value) or None, "recompute": int(recompute.value) or None}
+
+
+def proof_memory_plan_recompute_sharded(log_n, num_variables, num_constants, quotient_degree, config, world, lookup=None):
+    """bj_proof_memory_plan_recompute_sharded: device bytes of native_setup + prove on each of `world` GPUs on the recompute
+    plan, counted from the shapes (no device needed); at world 1 proof_memory_plan()["recompute"].  Chosen only after
+    Context.allow_sharded_recompute_plan.  Raises BoojumError for a world sharding rejects (cap_size < world,
+    world > 8 * LDE factor, row blocks of fewer than 2 rows)."""
+    c = native.Circuit()
+    c.log_n, c.num_variables, c.num_constants, c.quotient_degree = log_n, num_variables, num_constants, quotient_degree
+    c.fri_lde_factor, c.merkle_tree_cap_size = config.fri_lde_factor, config.merkle_tree_cap_size
+    c.security_level, c.pow_bits = config.security_level, config.pow_bits
+    if lookup:
+        c.lookup_width, c.lookup_num_repetitions = lookup["width"], lookup["num_repetitions"]
+    out = ctypes.c_uint64()
+    _ok(lib.bj_proof_memory_plan_recompute_sharded(ctypes.byref(c), world, ctypes.byref(out)), "bj_proof_memory_plan_recompute_sharded")
+    return int(out.value)
 
 
 def proof_memory_plan_lanes(log_n, num_variables, num_constants, quotient_degree, config, plan, n_lanes, lookup=None):

@@ -310,6 +310,12 @@ int32_t bj_ctx_allow_recompute_plan(bj_ctx* ctx, int32_t allow) {
   return BJ_OK;
 }
 
+int32_t bj_ctx_allow_sharded_recompute_plan(bj_ctx* ctx, int32_t allow) {
+  if (!ctx) return BJ_ERR_INVALID_ARG;
+  ctx->allow_sharded_recompute_plan = allow != 0;
+  return BJ_OK;
+}
+
 int32_t bj_ctx_memory_high_water(bj_ctx* ctx, uint64_t* bytes, int32_t reset) {
   bj::DeviceGuard device_guard(ctx);
   if (!ctx || !bytes) return BJ_ERR_INVALID_ARG;

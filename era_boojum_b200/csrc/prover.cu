@@ -106,36 +106,61 @@ struct NatSpan {
   u32 cnt;
 };
 
-// recompute plan (one GPU): the tree of oracle_build over the LDE at factor L of the spans' columns, built one committed coset
-// at a time.  Coset j is leaves [j n, (j + 1) n) (leaf t = j * n + row): its columns are evaluated into an n-row scratch per
-// column (bj_lde_cosets, the transforms of bj_lde), its leaves hashed into their slice, and the node levels are built once
-// the leaf array is complete, so the tree is bit-identical.  o.cols are the natural columns (they give the row length).
+// streamed and recompute plans: while the kernels of unit u run on a buffer that holds unit u alone, the context's shard is
+// the window of unit u; the caller's shard comes back on every exit path
+struct ShardWindow {
+  bj_ctx* ctx;
+  CosetShard saved;
+  ShardWindow(bj_ctx* c, u32 log_units, u32 u, u32 log_split) : ctx(c), saved(c->shard) { c->shard = CosetShard::window(log_units, u, log_split); }
+  ~ShardWindow() { ctx->shard = saved; }
+  ShardWindow(const ShardWindow&) = delete;
+  ShardWindow& operator=(const ShardWindow&) = delete;
+};
+
+// recompute plan: `cnt` columns of `in` (stride n; natural order, or monomials with from_monomials) evaluated on local unit k of
+// the committed domain alone into `out` (stride n >> split, the unit's rows).  One GPU: coset k (bj_lde_cosets).  Sharded:
+// bj_lde under the window of the rank's global unit k - the same coset transform, or fold + row-block transform, as the
+// resident sharded plan's LDE writes into local slot k, so every value is bit-identical to it.
+static int32_t lde_unit(bj_ctx* ctx, const uint64_t* in, uint64_t* out, u32 log_n, u32 log_l, u32 cnt, u64 k, int32_t from_monomials) {
+  if (cnt == 0) return BJ_OK;
+  if (comm_world(ctx) == 1) return bj_lde_cosets(ctx, in, 1ull << log_n, out, log_n, log_l, (u32)k, (u32)k + 1, cnt, from_monomials);
+  const u32 split = ctx->shard.log_split;
+  ShardWindow window(ctx, log_l + split, (u32)ctx->shard.global_unit(k), split);
+  return bj_lde(ctx, in, 1ull << log_n, out, log_n, log_l, cnt, from_monomials);
+}
+
+// recompute plan: the tree of oracle_build over the LDE at factor L of the spans' columns, built one committed unit at a time
+// (a coset on one GPU or a coset shard, a row block of nb = n / B rows on a split shard).  Local unit k is leaves
+// [k nb, (k + 1) nb) of this context's tree: its columns are evaluated into an nb-row scratch per column (lde_unit), its
+// leaves hashed into their slice, and the node levels are built once the leaf array is complete.  A unit is a whole subtree,
+// so the tree, its local cap and the cap exchange are those of oracle_build.  o.cols are the natural columns.
 static int32_t oracle_build_by_coset(bj_ctx* ctx, Oracle& o, const std::vector<NatSpan>& spans, u32 log_n, u32 log_l, u32 cap_size, u32 hasher) {
-  const u64 n = 1ull << log_n, n_leaves = n << log_l;
+  const u32 world = comm_world(ctx);
+  const u64 n = 1ull << log_n, nb = n >> ctx->shard.log_split, units = ctx->shard.local_units(1ull << log_l), n_leaves = units * nb;
   o.cols.clear();
   for (const NatSpan& sp : spans)
     for (u32 i = 0; i < sp.cnt; i++) o.cols.push_back(sp.p + (size_t)i * n);
   o.n_leaves = n_leaves;
-  o.cap_size = cap_size;
-  if (cap_size == 0 || n_leaves < cap_size) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "prover: oracle smaller than the cap");
+  o.cap_size = cap_size / world;
+  if (o.cap_size == 0 || n_leaves < o.cap_size) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "prover: oracle smaller than the cap");
   BJ_TRY(o.leaf_hashes.alloc(ctx, 4 * n_leaves));
   {
     DevMem ev;
-    BJ_TRY(ev.alloc(ctx, o.cols.size() * n));
-    std::vector<const uint64_t*> on_coset(o.cols.size());
-    for (size_t i = 0; i < on_coset.size(); i++) on_coset[i] = (const uint64_t*)ev.p + i * n;
-    for (u32 j = 0; j < (1u << log_l); j++) {
+    BJ_TRY(ev.alloc(ctx, o.cols.size() * nb));
+    std::vector<const uint64_t*> on_unit(o.cols.size());
+    for (size_t i = 0; i < on_unit.size(); i++) on_unit[i] = (const uint64_t*)ev.p + i * nb;
+    for (u64 k = 0; k < units; k++) {
       size_t c0 = 0;
       for (const NatSpan& sp : spans) {
-        if (sp.cnt) BJ_TRY(bj_lde_cosets(ctx, sp.p, n, (uint64_t*)ev.p + c0 * n, log_n, log_l, j, j + 1, sp.cnt, 0));
+        BJ_TRY(lde_unit(ctx, sp.p, (uint64_t*)ev.p + c0 * nb, log_n, log_l, sp.cnt, k, 0));
         c0 += sp.cnt;
       }
-      // the leaf phase alone: a tree of n leaves whose cap is its leaves
-      BJ_TRY(merkle_build(hasher)(ctx, on_coset.data(), (u32)on_coset.size(), n, 1, (u32)n, (uint64_t*)o.leaf_hashes.p + 4 * (size_t)j * n, nullptr));
+      // the leaf phase alone: a tree of nb leaves whose cap is its leaves
+      BJ_TRY(merkle_build(hasher)(ctx, on_unit.data(), (u32)on_unit.size(), nb, 1, (u32)nb, (uint64_t*)o.leaf_hashes.p + 4 * (size_t)k * nb, nullptr));
     }
   }
-  BJ_TRY(o.nodes.alloc(ctx, 4 * (n_leaves - cap_size)));
-  BJ_TRY(merkle_nodes(hasher)(ctx, o.leaf_hashes.p, n_leaves, cap_size, o.nodes.p));
+  BJ_TRY(o.nodes.alloc(ctx, 4 * (n_leaves - o.cap_size)));
+  BJ_TRY(merkle_nodes(hasher)(ctx, o.leaf_hashes.p, n_leaves, o.cap_size, o.nodes.p));
   return oracle_cap(ctx, o, cap_size, 1u << log_l);
 }
 
@@ -240,17 +265,6 @@ static int32_t keep_first_cosets_grouped(bj_ctx* ctx, ColumnGroups& g, std::vect
   return BJ_OK;
 }
 
-// streamed plan: while the quotient kernels of unit u run on a buffer that holds unit u alone, the context's shard is
-// the window of unit u; the caller's shard comes back on every exit path
-struct ShardWindow {
-  bj_ctx* ctx;
-  CosetShard saved;
-  ShardWindow(bj_ctx* c, u32 log_units, u32 u, u32 log_split) : ctx(c), saved(c->shard) { c->shard = CosetShard::window(log_units, u, log_split); }
-  ~ShardWindow() { ctx->shard = saved; }
-  ShardWindow(const ShardWindow&) = delete;
-  ShardWindow& operator=(const ShardWindow&) = delete;
-};
-
 int32_t copy_permutation_stage2_sharded(bj_ctx* ctx, const uint64_t* const* h_variable_cols, const uint64_t* const* h_sigma_cols, u32 n_cols,
                                         const uint64_t* h_non_residues, gl::e2 beta, gl::e2 gamma, u32 log_n, u32 chunk_size, u64* d_out);  // stage2.cu
 
@@ -324,9 +338,11 @@ struct QueryAnswer {
 // coset-sized scratch, from the natural-order columns (the stage-2 ones are kept for it).  On a sharded context each rank
 // keeps its units of the committed cosets and evaluates its own units of cosets [L, Q), one unit (a coset, or a row block
 // of one on a split shard, with its z(omega x) columns) at a time into a unit-sized scratch.  RECOMPUTE (one GPU, any Q and
-// L, opt-in) keeps no coset of the setup, witness and stage-2 columns at all: their trees are built one committed coset at a
+// L, opt-in; one GPU or sharded) keeps no coset of the setup, witness and stage-2 columns at all: their trees are built one committed coset at a
 // time (oracle_build_by_coset), the quotient runs the streamed plan's unit loop with no kept unit, the openings rebuild coset
-// 0 and DEEP and the queries cosets [0, L), all from the natural-order columns a chunk at a time.  The plan replays the
+// 0 and DEEP and the queries cosets [0, L), all from the natural-order columns a chunk at a time.  On a sharded context
+// (opt-in of its own) every rank does the same on its own units: its committed units for the trees, DEEP and the queries it
+// answers, its local slot 0 for the openings, its quotient units for the quotient.  The plan replays the
 // driver's stream-ordered pool allocations in order (pool_peak) and adds what the library keeps outside the pool
 // (library_reserve): twiddles, coset-power tables and the NTT scratch.
 enum MemoryPlan : u32 {
@@ -391,16 +407,16 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk, u64* setup
     m.add(4 * leaves);
     m.add(4 * (leaves - capl));
   };
-  auto tree_by_coset = [&](u64 cols) {  // oracle_build_by_coset: leaf hashes, one coset of the columns, then the nodes
+  auto tree_by_coset = [&](u64 cols) {  // oracle_build_by_coset: leaf hashes, one unit of the columns, then the nodes
     m.add(4 * leaves);
-    m.add(cols * n);
-    m.sub(cols * n);
+    m.add(cols * (n >> s.split));
+    m.sub(cols * (n >> s.split));
     m.add(4 * (leaves - capl));
   };
-  auto rebuild_chunks = [&]() {  // for_chunks: the monomials and one coset of a chunk of natural columns
+  auto rebuild_chunks = [&]() {  // for_chunks: the monomials and one unit (a coset, or a row block) of a chunk of natural columns
     m.add((u64)chunk * n);
-    m.add((u64)chunk * n);
-    m.sub((u64)chunk * n);
+    m.add((u64)chunk * (n >> s.split));
+    m.sub((u64)chunk * (n >> s.split));
     m.sub((u64)chunk * n);
   };
   auto lde_groups = [&](u32 cols) {  // lde_columns on a sharded context: at most two column groups of monomials at once
@@ -460,7 +476,7 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk, u64* setup
     m.add(s.n_s2 * nD);
     lde_groups(s.n_s2);
   }
-  const u64 zn = s.split && !streamed ? 2 * nD : 0;  // the streamed plan evaluates z(omega x) per unit, into its scratch
+  const u64 zn = s.split && !streamed && !recompute ? 2 * nD : 0;  // the streamed and recompute plans evaluate z(omega x) per unit, into their scratch
   if (zn) m.add(zn);
   // the compact plan keeps the natural stage-2 columns for DEEP and the queries, the streamed plan for the quotient, the
   // recompute plan for both
@@ -532,7 +548,7 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk, u64* setup
   m.sub((u64)s.n_queries * row_max);
   if (compact || recompute) {
     m.add((u64)chunk * n);
-    m.add((u64)chunk * n);
+    m.add((u64)chunk * (n >> s.split));
     m.add((u64)s.n_queries * chunk);
   }
   return m.peak;
@@ -551,6 +567,11 @@ static u64 library_reserve(const ProofShape& s) { return library_tables(s) + lan
 
 static bool compact_applies(const ProofShape& s) { return s.world == 1 && s.Q < s.L; }
 static bool recompute_applies(const ProofShape& s) { return s.world == 1; }
+// the recompute plan on `world` ranks: the shapes a sharded context takes (at most 8 row blocks per coset, at least 2 rows each)
+static bool sharded_shape_valid(const ProofShape& s) { return s.world <= 8 * s.L && s.log_n > s.split; }
+// ... where every rank owns a unit of the quotient's cosets [0, Q) (with Q < L and more ranks than Q units some own none;
+// the recompute plan is not taken there)
+static bool recompute_sharded_applies(const ProofShape& s) { return sharded_shape_valid(s) && ((u64)s.Q << s.split) >= s.world; }
 static bool streamed_applies(const ProofShape& s) { return s.Q > s.L; }  // on one GPU and on sharded contexts
 
 static u64 plan_bytes(const ProofShape& s, MemoryPlan plan, u32 chunk = 2) { return pool_peak(s, plan, chunk) + library_reserve(s); }
@@ -718,15 +739,17 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
   };
   {
     // the memory plan: resident if it fits under the limit, else compact (Q < L, one GPU), else streamed (Q > L), else
-    // recompute (one GPU, when the context allows it); refused before anything is launched.  On a sharded context every
-    // rank chooses under its own limit: the resident and streamed plans hold the same committed units and run the same
-    // collectives, so ranks on different plans still agree
+    // recompute (one GPU when the context allows it, a context with a communicator when it allows the sharded recompute
+    // plan); refused before anything is launched.  On a sharded context every rank chooses under its own limit: every plan
+    // commits to the same units and runs the same collectives, so ranks on different plans still agree
     ProofShape sh;
     BJ_TRY(proof_shape(*circuit, comm_world(ctx), &sh));
     s->plan[0] = plan_bytes(sh, PLAN_RESIDENT);
     s->plan[1] = compact_applies(sh) ? plan_bytes(sh, PLAN_COMPACT) : 0;
     s->plan[2] = streamed_applies(sh) ? plan_bytes(sh, PLAN_STREAMED) : 0;
-    s->plan[3] = ctx->allow_recompute_plan && recompute_applies(sh) ? plan_bytes(sh, PLAN_RECOMPUTE) : 0;
+    const bool recompute_allowed = (ctx->allow_recompute_plan && recompute_applies(sh)) ||
+                                   (ctx->allow_sharded_recompute_plan && ctx->comm && recompute_sharded_applies(sh));
+    s->plan[3] = recompute_allowed ? plan_bytes(sh, PLAN_RECOMPUTE) : 0;
     BJ_TRY(memory_limit(ctx, &s->limit));
     // with lanes alive on the context, a plan must also hold their proofs: one lane part each beside the plan
     const uint32_t lanes = ctx->lanes.load();
@@ -747,6 +770,29 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
       else
         BJ_FAIL(ctx, BJ_ERR_OOM, plan_message("bj_setup_create", need, s->limit) +
                                      (lanes ? " (each plan counted with the " + std::to_string(lanes) + " lane(s) of the context)" : std::string()));
+    }
+    if (ctx->comm && ctx->allow_sharded_recompute_plan && comm_world(ctx) > 1) {
+      // The resident and streamed plans share their LDEs' monomials (lde_columns: every rank interpolates a block of the
+      // columns, one all-gather per column group); the recompute plan evaluates its units from the natural-order columns and
+      // takes part in no such exchange.  So the ranks agree before their first collective: once one rank needs the recompute
+      // plan every rank takes it (a proof runs at its slowest rank's pace, so this costs the others no time), or, where a
+      // rank's limit does not hold it, every rank refuses.
+      const uint32_t world = comm_world(ctx);
+      const u64 mine[2] = {s->recompute ? 1u : 0u, fits(3) ? 1u : 0u};
+      std::vector<u64> all(2 * (size_t)world);
+      BJ_TRY(comm_all_gather_host(ctx->comm, mine, all.data(), 2));
+      bool any = false, every = true;
+      for (uint32_t r = 0; r < world; r++) {
+        any = any || all[2 * r];
+        every = every && all[2 * r + 1];
+      }
+      if (any && !every)
+        BJ_FAIL(ctx, BJ_ERR_OOM, "bj_setup_create: a rank needs the recompute plan and another rank's limit does not hold it; " +
+                                     plan_message("this rank", need, s->limit));
+      if (any) {
+        s->streamed = false;
+        s->recompute = true;
+      }
     }
     if (s->compact || s->recompute) {
       // wider recompute chunks only save kernel launches: the chunk grows into at most half of the headroom the limit leaves
@@ -873,7 +919,7 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   const u64 Qn = n * Q;  // compact plan: elements of a setup / witness / stage-2 column kept on the device (cosets [0, Q))
   const uint32_t log_kept = streamed ? log_l : log_d;  // streamed plan: those columns are evaluated on the cosets [0, L) only
   const u64 nK = streamed ? nL : nD;      // stride of those columns on the resident and streamed plans
-  if (setup->col_len != (compact ? Qn : recompute ? 0 : nK) || (recompute && world > 1))
+  if (setup->col_len != (compact ? Qn : recompute ? 0 : nK))
     BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: the setup was built with a different shard");
   const uint32_t chunk = setup->chunk;  // compact and recompute plans: natural-order columns recomputed at a time
   // the compact plan keeps cosets [0, Q) of the setup, witness and stage-2 columns, the recompute plan none: DEEP and the
@@ -1007,9 +1053,9 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   }
   // a row block of a split shard does not hold z(omega x) (another block of the coset does).  On a unit with shift sigma,
   // z(omega x) is the LDE of z on the shift sigma * omega in the same row order: two more columns (c0, c1 of z).  The
-  // streamed plan evaluates them one unit at a time with the quotient's other columns.
+  // streamed and recompute plans evaluate them one unit at a time with the quotient's other columns.
   DevMem z_next;
-  if (split && !streamed && ctx->shard.local_units(Q)) {
+  if (split && !streamed && !recompute && ctx->shard.local_units(Q)) {
     BJ_TRY(z_next.alloc(ctx, 2 * nD));
     BJ_TRY(bj_lde_next_row(ctx, (const uint64_t*)st2.p, n, (uint64_t*)z_next.p, log_n, log_d, 2, 0));
   }
@@ -1248,11 +1294,11 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     for (uint32_t j = 0; j < n_s2; j += 2) pair_start[S + w_or.cols.size() + j] = 1;
   }
   // chunks of `chunk` natural columns among nat[lo, hi) (an Fp2 pair never split): monomials by one iNTT, then body(c0, cnt,
-  // monomials, scratch for one coset of the chunk)
+  // monomials, scratch for one unit of the chunk: a coset, or nb rows of one on a split shard, stride nb)
   auto for_chunks = [&](uint32_t lo, uint32_t hi, const std::function<int32_t(uint32_t, uint32_t, const uint64_t*, uint64_t*)>& body) -> int32_t {
     DevMem mono, ev;
     BJ_TRY(mono.alloc(ctx, (size_t)chunk * n));
-    BJ_TRY(ev.alloc(ctx, (size_t)chunk * n));
+    BJ_TRY(ev.alloc(ctx, (size_t)chunk * nb));
     for (uint32_t c0 = lo; c0 < hi;) {
       uint32_t cnt = std::min<uint32_t>(chunk, hi - c0);
       if (c0 + cnt < hi && pair_start[c0 + cnt - 1]) cnt--;
@@ -1264,8 +1310,9 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     }
     return BJ_OK;
   };
-  // recompute plan: the barycentric sums of the natural columns among flat from coset 0, rebuilt a chunk at a time (only the
-  // chunks that hold one of them), those of the quotient oracle's columns directly
+  // recompute plan: the barycentric sums of the natural columns among flat from local slot 0 (coset 0 on one GPU, this rank's
+  // coset or row block on a sharded context), rebuilt a chunk at a time (only the chunks that hold one of them), those of the
+  // quotient oracle's columns directly
   auto open_rebuilt = [&](const std::vector<const uint64_t*>& flat, const uint64_t a[2], uint64_t* ev) -> int32_t {
     auto evaluate = [&](const std::vector<const uint64_t*>& cols, const std::vector<size_t>& at) -> int32_t {
       if (cols.empty()) return BJ_OK;
@@ -1292,13 +1339,13 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     }
     BJ_TRY(evaluate(direct, direct_at));
     return for_chunks(lo, hi, [&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* on_coset) -> int32_t {
-      BJ_TRY(bj_lde_cosets(ctx, mono, n, on_coset, log_n, log_l, 0, 1, cnt, 1));
+      BJ_TRY(lde_unit(ctx, mono, on_coset, log_n, log_l, cnt, 0, 1));
       std::vector<const uint64_t*> cols;
       std::vector<size_t> at;
       for (size_t i = 0; i < flat.size(); i++) {
         const auto it = nat_of.find(flat[i]);
         if (it == nat_of.end() || it->second < c0 || it->second >= c0 + cnt) continue;
-        cols.push_back(on_coset + (size_t)(it->second - c0) * n);
+        cols.push_back(on_coset + (size_t)(it->second - c0) * nb);
         at.push_back(i);
       }
       return evaluate(cols, at);
@@ -1314,19 +1361,21 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     if (flat.empty()) return BJ_OK;
     std::vector<uint64_t> ev(2 * flat.size());
     const uint64_t a[2] = {at.c0, at.c1};
-    if (recompute) {
-      BJ_TRY(open_rebuilt(flat, a, ev.data()));
-    } else if (world == 1) {
-      BJ_TRY(bj_barycentric_evaluate(ctx, flat.data(), (uint32_t)flat.size(), log_n, a, ev.data()));
+    if (world == 1) {
+      if (recompute) BJ_TRY(open_rebuilt(flat, a, ev.data()));
+      else BJ_TRY(bj_barycentric_evaluate(ctx, flat.data(), (uint32_t)flat.size(), log_n, a, ev.data()));
     } else {
       // the columns are split over the coset groups: ranks [g B, (g + 1) B) hold the B row blocks of coset g (B = 1: one rank,
-      // its whole coset) and open column block g from it, each rank its block's contribution.  The contributions are
-      // gathered and the B of a group summed.
+      // its whole coset) and open column block g from it, each rank its block's contribution (on the recompute plan from its
+      // rebuilt local slot 0).  The contributions are gathered and the B of a group summed.
       const uint32_t groups = world >> split, g = rank >> split;
       const size_t per = (flat.size() + groups - 1) / groups, first = std::min(flat.size(), (size_t)g * per);
       const size_t cnt = std::min(per, flat.size() - first);
       std::vector<uint64_t> mine(2 * per, 0), all(2 * per * world);
-      if (cnt) BJ_TRY(bj_barycentric_evaluate(ctx, flat.data() + first, (uint32_t)cnt, log_n, a, mine.data()));
+      if (cnt && recompute)
+        BJ_TRY(open_rebuilt(std::vector<const uint64_t*>(flat.begin() + first, flat.begin() + first + cnt), a, mine.data()));
+      else if (cnt)
+        BJ_TRY(bj_barycentric_evaluate(ctx, flat.data() + first, (uint32_t)cnt, log_n, a, mine.data()));
       BJ_TRY(comm_all_gather_host(ctx->comm, (const u64*)mine.data(), (u64*)all.data(), 2 * per));
       for (uint32_t gg = 0; gg < groups; gg++)
         for (size_t e = 0; e < 2 * per && gg * 2 * per + e < ev.size(); e++) {
@@ -1400,7 +1449,9 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     const uint64_t* chs;
   };
   std::vector<DeepGroup> deep_groups;
-  // sources i of a group with keep(i) on the points [first, first + count), column pointers moved by col_off(i)
+  // sources i of a group with keep(i) on the local points [first, first + count), column pointers moved by at_col.  One GPU:
+  // any run of points.  Sharded (recompute plan): the whole local domain, or local unit k (first = k nb, count = nb) under
+  // its window, whose points the kernel then places at their global indices.
   auto deep_range = [&](const DeepGroup& g, const std::function<bool(size_t)>& keep, const std::function<const uint64_t*(const uint64_t*)>& at_col,
                         u64 first, u64 count) -> int32_t {
     std::vector<const uint64_t*> p0, p1;
@@ -1417,8 +1468,13 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     }
     if (p0.empty()) return BJ_OK;
     const uint64_t a[2] = {g.at.c0, g.at.c1};
-    return bj_deep_quotient_range(ctx, p0.data(), p1.data(), (uint32_t)p0.size(), v.data(), ch.data(), a, log_n + log_l, first, count,
-                                  (uint64_t*)deep.p + first, (uint64_t*)deep.p + nL + first);
+    uint64_t *acc0 = (uint64_t*)deep.p + first, *acc1 = (uint64_t*)deep.p + nL + first;
+    if (world == 1)
+      return bj_deep_quotient_range(ctx, p0.data(), p1.data(), (uint32_t)p0.size(), v.data(), ch.data(), a, log_n + log_l, first, count, acc0, acc1);
+    if (count == nL)
+      return bj_deep_quotient_group(ctx, p0.data(), p1.data(), (uint32_t)p0.size(), v.data(), ch.data(), a, log_n + log_l, acc0, acc1);
+    ShardWindow window(ctx, log_l + split, (u32)ctx->shard.global_unit(first / nb), split);
+    return bj_deep_quotient_group(ctx, p0.data(), p1.data(), (uint32_t)p0.size(), v.data(), ch.data(), a, log_n + log_l, acc0, acc1);
   };
   auto deep_group = [&](const std::vector<Src>& srcs, const std::vector<gl::e2>& vals, gl::e2 at, const uint64_t* chs) -> int32_t {
     if (srcs.empty()) return BJ_OK;
@@ -1452,17 +1508,19 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
       off += g.srcs.size();
     }
   }
-  if (compact || recompute)  // cosets [first_rebuilt, L): every chunk of natural columns evaluated on one coset at a time, its DEEP terms added
+  // local units of the committed cosets [0, L): the cosets themselves on one GPU, this rank's units on a sharded context
+  const u64 units_l = ctx->shard.local_units(L);
+  if (compact || recompute)  // units [first_rebuilt, units_l): every chunk of natural columns evaluated on one unit at a time, its DEEP terms added
     BJ_TRY(for_chunks(0, (uint32_t)nat.size(), [&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* ev) -> int32_t {
       auto in_chunk = [&](const uint64_t* p) {
         const auto it = nat_of.find(p);
         return it != nat_of.end() && it->second >= c0 && it->second < c0 + cnt;
       };
-      auto on_coset = [&](const uint64_t* p) -> const uint64_t* { return ev + (size_t)(nat_of.at(p) - c0) * n; };
-      for (uint32_t j = first_rebuilt; j < L; j++) {
-        BJ_TRY(bj_lde_cosets(ctx, mono, n, ev, log_n, log_l, j, j + 1, cnt, 1));
+      auto on_unit = [&](const uint64_t* p) -> const uint64_t* { return ev + (size_t)(nat_of.at(p) - c0) * nb; };
+      for (u64 k = first_rebuilt; k < units_l; k++) {
+        BJ_TRY(lde_unit(ctx, mono, ev, log_n, log_l, cnt, k, 1));
         for (const DeepGroup& g : deep_groups)
-          BJ_TRY(deep_range(g, [&](size_t i) { return in_chunk((*g.srcs)[i].c0); }, on_coset, (u64)j * n, n));
+          BJ_TRY(deep_range(g, [&](size_t i) { return in_chunk((*g.srcs)[i].c0); }, on_unit, k * nb, nb));
       }
       return BJ_OK;
     }));
@@ -1542,26 +1600,34 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     parts.push_back(std::move(path));
   }
   if (compact || recompute) {
-    // queries whose leaf lies in a coset j >= first_rebuilt: one recompute of each such coset per chunk, the queried rows
-    // gathered from it (the rows of every query, so that the gather buffer is the one the plan counts).  Natural column i
-    // belongs to the setup (rows in parts[6]), witness (parts[0]) or stage-2 (parts[2]) oracle.
-    std::vector<std::vector<uint32_t>> by_coset(L);
+    // queries this context answers whose leaf lies in a local unit k >= first_rebuilt (a coset on one GPU): one recompute of
+    // each such unit per chunk, the queried rows gathered from it (the rows of every query, so that the gather buffer is the
+    // one the plan counts).  Natural column i belongs to the setup (rows in parts[6]), witness (parts[0]) or stage-2
+    // (parts[2]) oracle.  On a sharded context every rank runs the pass, also one that answers none of these queries: its
+    // peers are rebuilding meanwhile and the exchange waits for them, so it gathers from the chunk's monomials instead, and
+    // every rank's pool reaches the peak its plan counts.
+    const u32 log_nb = log_n - split;
+    std::vector<std::vector<uint32_t>> by_unit(units_l);
     for (uint32_t q = 0; q < num_queries; q++)
-      if (idxs[q] >= Fn) by_coset[idxs[q] / n].push_back(q);
+      if (owner[q] == rank && (loc_idx[q] >> log_nb) >= first_rebuilt) by_unit[loc_idx[q] >> log_nb].push_back(q);
     bool any = false;
-    for (uint32_t j = first_rebuilt; j < L; j++) any = any || !by_coset[j].empty();
+    for (const auto& qs : by_unit) any = any || !qs.empty();
     const uint32_t Wc = (uint32_t)w_or.cols.size();
-    if (any)
+    if (any || world > 1)
       BJ_TRY(for_chunks(0, (uint32_t)nat.size(), [&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* ev) -> int32_t {
         std::vector<const uint64_t*> cols(cnt);
-        for (uint32_t i = 0; i < cnt; i++) cols[i] = ev + (size_t)i * n;
-        for (uint32_t j = first_rebuilt; j < L; j++) {
-          const auto& qs = by_coset[j];
+        std::vector<uint64_t> rows_in(num_queries, 0), got((size_t)num_queries * cnt);
+        if (!any) {
+          for (uint32_t i = 0; i < cnt; i++) cols[i] = mono + (size_t)i * n;
+          return bj_query_leaf_elements(ctx, cols.data(), cnt, 1, n, rows_in.data(), num_queries, got.data());
+        }
+        for (uint32_t i = 0; i < cnt; i++) cols[i] = ev + (size_t)i * nb;
+        for (u64 k = first_rebuilt; k < units_l; k++) {
+          const auto& qs = by_unit[k];
           if (qs.empty()) continue;
-          BJ_TRY(bj_lde_cosets(ctx, mono, n, ev, log_n, log_l, j, j + 1, cnt, 1));
-          std::vector<uint64_t> rows_in(num_queries, 0), got((size_t)num_queries * cnt);
-          for (uint32_t q : qs) rows_in[q] = idxs[q] - (u64)j * n;
-          BJ_TRY(bj_query_leaf_elements(ctx, cols.data(), cnt, 1, n, rows_in.data(), num_queries, got.data()));
+          BJ_TRY(lde_unit(ctx, mono, ev, log_n, log_l, cnt, k, 1));
+          for (uint32_t q : qs) rows_in[q] = loc_idx[q] & (nb - 1);
+          BJ_TRY(bj_query_leaf_elements(ctx, cols.data(), cnt, 1, nb, rows_in.data(), num_queries, got.data()));
           for (uint32_t i = 0; i < cnt; i++) {
             const uint32_t col = c0 + i;
             Part& pt = col < S ? parts[6] : col < S + Wc ? parts[0] : parts[2];
@@ -1722,6 +1788,16 @@ int32_t bj_proof_memory_plan_recompute(const bj_circuit* circuit, uint32_t world
   if (!out) return BJ_ERR_INVALID_ARG;
   BJ_TRY(memory_plan_shape(circuit, world, &sh));
   *out = recompute_applies(sh) ? plan_bytes(sh, PLAN_RECOMPUTE) : 0;
+  return BJ_OK;
+}
+
+int32_t bj_proof_memory_plan_recompute_sharded(const bj_circuit* circuit, uint32_t world, uint64_t* out) {
+  ProofShape sh;
+  if (!out) return BJ_ERR_INVALID_ARG;
+  *out = 0;
+  BJ_TRY(memory_plan_shape(circuit, world, &sh));
+  if (!sharded_shape_valid(sh)) return BJ_ERR_INVALID_ARG;
+  *out = recompute_sharded_applies(sh) ? plan_bytes(sh, PLAN_RECOMPUTE) : 0;
   return BJ_OK;
 }
 

@@ -51,6 +51,7 @@ SIGNATURES = {
     "bj_launch_count": (_u64, [_vp]),
     "bj_ctx_set_memory_limit": (_i32, [_vp, _u64]),
     "bj_ctx_allow_recompute_plan": (_i32, [_vp, _i32]),
+    "bj_ctx_allow_sharded_recompute_plan": (_i32, [_vp, _i32]),
     "bj_ctx_memory_high_water": (_i32, [_vp, _vp, _i32]),
     "bj_ctx_create_lane": (_i32, [_vp, _pp]),
     "bj_alloc": (_i32, [_vp, _sz, _pp]),
@@ -131,6 +132,7 @@ SIGNATURES = {
     "bj_proof_memory_plan_streamed": (_i32, [_vp, _u32, _vp]),
     "bj_proof_memory_plan_streamed_sharded": (_i32, [_vp, _u32, _vp]),
     "bj_proof_memory_plan_recompute": (_i32, [_vp, _u32, _vp]),
+    "bj_proof_memory_plan_recompute_sharded": (_i32, [_vp, _u32, _vp]),
     "bj_setup_is_compact": (_i32, [_vp]),
     "bj_setup_plan": (_i32, [_vp]),
     "bj_setup_memory_plan": (_i32, [_vp, _vp]),

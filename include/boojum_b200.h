@@ -80,17 +80,26 @@ BJ_API uint64_t bj_launch_count(const bj_ctx* ctx);
 /* Device-memory limit of the prover driver on this context (bytes; 0, the default: what the device has free when
  * bj_setup_create runs, plus what the context's pool holds without using it).  bj_setup_create compares the memory plans of
  * bj_proof_memory_plan and bj_proof_memory_plan_streamed(_sharded) with it: RESIDENT if that fits, else COMPACT (one GPU,
- * quotient degree < LDE factor), else STREAMED (quotient degree > LDE factor, one GPU or sharded), else RECOMPUTE (one GPU, only
- * after bj_ctx_allow_recompute_plan(ctx, 1)), else BJ_ERR_OOM with every applicable byte count in the message and no kernel
- * launched.  With quotient degree = LDE factor only RESIDENT (and the opt-in RECOMPUTE) applies.  On
- * a sharded context every rank chooses under its own limit; ranks on different plans still return the same proof.  bj_prove
- * follows the setup's plan and refuses the same way if the limit was lowered below it since. */
+ * quotient degree < LDE factor), else STREAMED (quotient degree > LDE factor, one GPU or sharded), else RECOMPUTE (one GPU only
+ * after bj_ctx_allow_recompute_plan(ctx, 1); a context with a communicator only after bj_ctx_allow_sharded_recompute_plan(ctx,
+ * 1), counted by bj_proof_memory_plan_recompute_sharded), else BJ_ERR_OOM with every applicable byte count in the message and
+ * no kernel launched.  With quotient degree = LDE factor only RESIDENT (and the opt-in RECOMPUTE) applies.  On a sharded
+ * context every rank chooses under its own limit; ranks on different plans (resident, streamed, recompute) still return the
+ * same proof.  bj_prove follows the setup's plan and refuses the same way if the limit was lowered below it since. */
 BJ_API int32_t bj_ctx_set_memory_limit(bj_ctx* ctx, uint64_t bytes);
 /* allow != 0 lets bj_setup_create fall back to the RECOMPUTE plan (bj_proof_memory_plan_recompute) when none of RESIDENT,
  * COMPACT and STREAMED fits under the limit; the refusal below every plan then names the recompute bytes too.  Off by default:
  * the recompute plan rebuilds every coset of the setup, witness and stage-2 columns wherever it is read, so it is slower, and
  * a caller that relies on BJ_ERR_OOM below the smaller plans keeps it.  A sharded context ignores the switch. */
 BJ_API int32_t bj_ctx_allow_recompute_plan(bj_ctx* ctx, int32_t allow);
+/* allow != 0 lets bj_setup_create on a context with a communicator fall back to the RECOMPUTE plan on this rank
+ * (bj_proof_memory_plan_recompute_sharded) when neither RESIDENT nor STREAMED fits under the rank's limit; the refusal below
+ * every plan then names the recompute bytes too.  Off by default, for the reasons of bj_ctx_allow_recompute_plan, which a
+ * sharded context still ignores.  Set it alike on every rank: with it on, the ranks exchange their choice before their first
+ * collective, and once one rank needs the recompute plan every rank takes it (the resident and streamed plans share LDE
+ * monomials the recompute plan does not compute), or every rank refuses with BJ_ERR_OOM where a rank's limit does not hold
+ * it.  A context without a communicator ignores this switch. */
+BJ_API int32_t bj_ctx_allow_sharded_recompute_plan(bj_ctx* ctx, int32_t allow);
 /* highest device memory the context's pool has had in use (cudaMemPoolAttrUsedMemHigh); reset != 0 restarts the mark.
  * Synchronises.  Memory the library keeps outside the pool (twiddles, coset-power tables, scratch) is not included. */
 BJ_API int32_t bj_ctx_memory_high_water(bj_ctx* ctx, uint64_t* bytes, int32_t reset);
@@ -541,6 +550,18 @@ BJ_API int32_t bj_proof_memory_plan_streamed_sharded(const bj_circuit* circuit, 
  * rebuild cosets [0, L) the same way.  Proofs are bit-identical to the resident plan's; opt in with
  * bj_ctx_allow_recompute_plan. */
 BJ_API int32_t bj_proof_memory_plan_recompute(const bj_circuit* circuit, uint32_t world, uint64_t* out);
+/* The RECOMPUTE plan's bytes on each of `world` GPUs, counted like bj_proof_memory_plan_streamed_sharded (at world 1 the value
+ * of bj_proof_memory_plan_recompute), for any quotient degree.  Each rank keeps no coset of the setup, witness or stage-2
+ * columns and works on its own units u = rank (mod world) - whole cosets on a coset shard (world <= L), row blocks of
+ * n * L / world rows on a split shard: it builds each tree one of its committed units at a time (the unit's columns
+ * evaluated from natural order into a unit-sized scratch, its leaves hashed into their slice), evaluates every column the
+ * quotient reads onto one of its quotient units at a time (with the unit's z(omega x) columns on a split shard), rebuilds its
+ * local slot 0 a chunk of columns at a time for the openings, and its committed units for DEEP and for the queries it
+ * answers.  The gathered quotient, the collectives and the proof are unchanged.  *out = 0 where some rank would own no
+ * quotient unit (Q < L and world > Q: the plan does not apply there).  *out = 0 and BJ_ERR_INVALID_ARG for the
+ * shapes sharding rejects: cap_size < world, world > 8 * LDE factor, a row block of fewer than 2 rows.  Chosen only after
+ * bj_ctx_allow_sharded_recompute_plan. */
+BJ_API int32_t bj_proof_memory_plan_recompute_sharded(const bj_circuit* circuit, uint32_t world, uint64_t* out);
 /* 1 if bj_setup_create chose the compact plan, 0 otherwise (resident, streamed or recompute) */
 BJ_API int32_t bj_setup_is_compact(const bj_setup* setup);
 /* the plan bj_setup_create chose: BJ_PLAN_RESIDENT, BJ_PLAN_COMPACT, BJ_PLAN_STREAMED or BJ_PLAN_RECOMPUTE */
