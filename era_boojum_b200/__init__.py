@@ -268,6 +268,13 @@ class Context:
         other plan fits under the limit.  Off by default; a sharded context ignores it."""
         self._check(lib.bj_ctx_allow_recompute_plan(self._h, int(bool(allow))))
 
+    def set_max_row_blocks(self, max_blocks):
+        """bj_ctx_set_max_row_blocks: row blocks per coset (1, the default, 2, 4 or 8) the one-GPU recompute plan may cut its
+        trees and quotient into.  When native_setup takes the recompute plan it takes the fewest row blocks whose plan
+        (proof_memory_plan_recompute_blocks) fits; NativeSetup.row_blocks reports them.  A context with a communicator ignores
+        it; lanes inherit it."""
+        self._check(lib.bj_ctx_set_max_row_blocks(self._h, int(max_blocks)))
+
     def allow_sharded_recompute_plan(self, allow=True):
         """bj_ctx_allow_sharded_recompute_plan: with allow, native_setup on a context with a communicator falls back to the
         recompute plan on this rank (proof_memory_plan_recompute_sharded) when neither the resident nor the streamed plan fits
@@ -747,11 +754,28 @@ def proof_memory_plan_recompute_sharded(log_n, num_variables, num_constants, quo
     return int(out.value)
 
 
-def proof_memory_plan_lanes(log_n, num_variables, num_constants, quotient_degree, config, plan, n_lanes, lookup=None):
-    """bj_proof_memory_plan_lanes_host: device bytes of one setup proved on n_lanes lanes at once on one GPU, on `plan`
-    ("resident", "compact", "streamed" or "recompute"), counted from the shapes (no device needed) -> dict(setup=bytes the
-    setup and the shared tables hold, lane=bytes each lane adds, total=setup + n_lanes * lane), or None where the plan does
-    not apply.  At one lane, total is proof_memory_plan()[plan]."""
+def proof_memory_plan_recompute_blocks(log_n, num_variables, num_constants, quotient_degree, config, blocks, lookup=None):
+    """bj_proof_memory_plan_recompute_blocks: device bytes of native_setup + prove on one GPU on the recompute plan with every
+    coset cut into `blocks` row blocks (1, 2, 4 or 8) in the trees and the quotient, counted from the shapes (no device
+    needed); at blocks = 1 proof_memory_plan()["recompute"].  Raises BoojumError for other block counts and for row blocks of
+    fewer than 2 rows."""
+    c = native.Circuit()
+    c.log_n, c.num_variables, c.num_constants, c.quotient_degree = log_n, num_variables, num_constants, quotient_degree
+    c.fri_lde_factor, c.merkle_tree_cap_size = config.fri_lde_factor, config.merkle_tree_cap_size
+    c.security_level, c.pow_bits = config.security_level, config.pow_bits
+    if lookup:
+        c.lookup_width, c.lookup_num_repetitions = lookup["width"], lookup["num_repetitions"]
+    out = ctypes.c_uint64()
+    _ok(lib.bj_proof_memory_plan_recompute_blocks(ctypes.byref(c), blocks, ctypes.byref(out)), "bj_proof_memory_plan_recompute_blocks")
+    return int(out.value)
+
+
+def proof_memory_plan_lanes(log_n, num_variables, num_constants, quotient_degree, config, plan, n_lanes, lookup=None, row_blocks=1):
+    """bj_proof_memory_plan_lanes_host(_blocks): device bytes of one setup proved on n_lanes lanes at once on one GPU, on `plan`
+    ("resident", "compact", "streamed" or "recompute", the last with row_blocks row blocks per coset), counted from the shapes
+    (no device needed) -> dict(setup=bytes the setup and the shared tables hold, lane=bytes each lane adds, total=setup +
+    n_lanes * lane), or None where the plan does not apply.  At one lane, total is proof_memory_plan()[plan] (and
+    proof_memory_plan_recompute_blocks for row_blocks > 1)."""
     c = native.Circuit()
     c.log_n, c.num_variables, c.num_constants, c.quotient_degree = log_n, num_variables, num_constants, quotient_degree
     c.fri_lde_factor, c.merkle_tree_cap_size = config.fri_lde_factor, config.merkle_tree_cap_size
@@ -761,7 +785,7 @@ def proof_memory_plan_lanes(log_n, num_variables, num_constants, quotient_degree
     kind = {"resident": native.PLAN_RESIDENT, "compact": native.PLAN_COMPACT, "streamed": native.PLAN_STREAMED,
             "recompute": native.PLAN_RECOMPUTE}[plan]
     out = (ctypes.c_uint64 * 3)()
-    _ok(lib.bj_proof_memory_plan_lanes_host(ctypes.byref(c), kind, n_lanes, out), "bj_proof_memory_plan_lanes_host")
+    _ok(lib.bj_proof_memory_plan_lanes_host_blocks(ctypes.byref(c), kind, row_blocks, n_lanes, out), "bj_proof_memory_plan_lanes_host_blocks")
     return {"setup": int(out[0]), "lane": int(out[1]), "total": int(out[2])} if out[2] else None
 
 
@@ -910,6 +934,14 @@ class NativeSetup:
         _ok(min(k, 0), "bj_setup_plan")
         return {native.PLAN_RESIDENT: "resident", native.PLAN_COMPACT: "compact", native.PLAN_STREAMED: "streamed",
                 native.PLAN_RECOMPUTE: "recompute"}[k]
+
+    @property
+    def row_blocks(self):
+        """the row blocks per coset bj_setup_create chose for the recompute plan on one GPU (bj_setup_row_blocks); 1 on every
+        other plan"""
+        k = lib.bj_setup_row_blocks(self._h)
+        _ok(min(k, 0), "bj_setup_row_blocks")
+        return int(k)
 
     def memory_plan(self):
         """bj_setup_memory_plan: the chosen plan -> dict(pool=peak pool bytes of setup + prove, outside_pool=bound on the

@@ -95,6 +95,7 @@ int32_t ctx_new_lane(bj_ctx* parent, bj_ctx** out) {
   lane->ntt_bulk = parent->ntt_bulk;
   lane->memory_limit = parent->memory_limit;
   lane->allow_recompute_plan = parent->allow_recompute_plan;
+  lane->max_row_blocks = parent->max_row_blocks;
   lane->own_twiddles = false;
   BJ_CUDA(parent, cudaStreamCreateWithFlags(&lane->stream, cudaStreamNonBlocking));
   lane->own_stream = true;
@@ -307,6 +308,14 @@ int32_t bj_ctx_set_memory_limit(bj_ctx* ctx, uint64_t bytes) {
 int32_t bj_ctx_allow_recompute_plan(bj_ctx* ctx, int32_t allow) {
   if (!ctx) return BJ_ERR_INVALID_ARG;
   ctx->allow_recompute_plan = allow != 0;
+  return BJ_OK;
+}
+
+int32_t bj_ctx_set_max_row_blocks(bj_ctx* ctx, uint32_t max_blocks) {
+  if (!ctx) return BJ_ERR_INVALID_ARG;
+  if (max_blocks == 0 || max_blocks > 8 || (max_blocks & (max_blocks - 1)))
+    BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_ctx_set_max_row_blocks: 1, 2, 4 or 8 row blocks per coset");
+  ctx->max_row_blocks = max_blocks;
   return BJ_OK;
 }
 

@@ -142,6 +142,7 @@ struct bj_ctx {
   uint64_t memory_limit = 0;   // bj_ctx_set_memory_limit: device bytes a proof may use (0: what is free when the setup is created)
   bool allow_recompute_plan = false;  // bj_ctx_allow_recompute_plan: bj_setup_create may fall back to the recompute plan (one GPU)
   bool allow_sharded_recompute_plan = false;  // bj_ctx_allow_sharded_recompute_plan: the same on a context with a communicator
+  uint32_t max_row_blocks = 1;  // bj_ctx_set_max_row_blocks: row blocks per coset the one-GPU recompute plan may cut its units into
   unsigned long long* pow_best = nullptr;  // bj_pow_blake2s's one-word result, allocated on first use
   void* gate_program = nullptr;            // a long gate program's device copy (gates.cu), grown on demand, kept
   size_t gate_program_bytes = 0;

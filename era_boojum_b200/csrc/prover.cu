@@ -118,25 +118,28 @@ struct ShardWindow {
 };
 
 // recompute plan: `cnt` columns of `in` (stride n; natural order, or monomials with from_monomials) evaluated on local unit k of
-// the committed domain alone into `out` (stride n >> split, the unit's rows).  One GPU: coset k (bj_lde_cosets).  Sharded:
-// bj_lde under the window of the rank's global unit k - the same coset transform, or fold + row-block transform, as the
-// resident sharded plan's LDE writes into local slot k, so every value is bit-identical to it.
-static int32_t lde_unit(bj_ctx* ctx, const uint64_t* in, uint64_t* out, u32 log_n, u32 log_l, u32 cnt, u64 k, int32_t from_monomials) {
+// the committed domain alone into `out` (stride n >> split, the unit's rows).  One GPU: coset k (bj_lde_cosets), or, with
+// 2^rb row blocks per coset, row block k % 2^rb of coset k >> rb.  Sharded (rb = 0): the rank's global unit k.  A row block
+// or a sharded unit goes through bj_lde under the unit's window - the same coset transform, or fold + row-block transform,
+// as the resident sharded plan's LDE writes into local slot k, so every value is bit-identical to the resident plan's.
+static int32_t lde_unit(bj_ctx* ctx, const uint64_t* in, uint64_t* out, u32 log_n, u32 log_l, u32 cnt, u64 k, int32_t from_monomials, u32 rb = 0) {
   if (cnt == 0) return BJ_OK;
-  if (comm_world(ctx) == 1) return bj_lde_cosets(ctx, in, 1ull << log_n, out, log_n, log_l, (u32)k, (u32)k + 1, cnt, from_monomials);
-  const u32 split = ctx->shard.log_split;
-  ShardWindow window(ctx, log_l + split, (u32)ctx->shard.global_unit(k), split);
+  const u32 split = ctx->shard.log_split + rb;
+  if (comm_world(ctx) == 1 && split == 0) return bj_lde_cosets(ctx, in, 1ull << log_n, out, log_n, log_l, (u32)k, (u32)k + 1, cnt, from_monomials);
+  ShardWindow window(ctx, log_l + split, (u32)ctx->shard.global_unit(k), split);  // one GPU: global_unit(k) = k
   return bj_lde(ctx, in, 1ull << log_n, out, log_n, log_l, cnt, from_monomials);
 }
 
 // recompute plan: the tree of oracle_build over the LDE at factor L of the spans' columns, built one committed unit at a time
-// (a coset on one GPU or a coset shard, a row block of nb = n / B rows on a split shard).  Local unit k is leaves
-// [k nb, (k + 1) nb) of this context's tree: its columns are evaluated into an nb-row scratch per column (lde_unit), its
-// leaves hashed into their slice, and the node levels are built once the leaf array is complete.  A unit is a whole subtree,
-// so the tree, its local cap and the cap exchange are those of oracle_build.  o.cols are the natural columns.
-static int32_t oracle_build_by_coset(bj_ctx* ctx, Oracle& o, const std::vector<NatSpan>& spans, u32 log_n, u32 log_l, u32 cap_size, u32 hasher) {
+// (a coset on one GPU or a coset shard, a row block of nb = n / B rows on a split shard or, with rb > 0, on one GPU cutting
+// each coset into B = 2^rb row blocks).  Local unit k is leaves [k nb, (k + 1) nb) of this context's tree: its columns are
+// evaluated into an nb-row scratch per column (lde_unit), its leaves hashed into their slice, and the node levels are built
+// once the leaf array is complete.  A unit is a whole subtree, so the tree, its local cap and the cap exchange are those of
+// oracle_build.  o.cols are the natural columns.
+static int32_t oracle_build_by_coset(bj_ctx* ctx, Oracle& o, const std::vector<NatSpan>& spans, u32 log_n, u32 log_l, u32 cap_size, u32 hasher,
+                                     u32 rb) {
   const u32 world = comm_world(ctx);
-  const u64 n = 1ull << log_n, nb = n >> ctx->shard.log_split, units = ctx->shard.local_units(1ull << log_l), n_leaves = units * nb;
+  const u64 n = 1ull << log_n, nb = n >> (ctx->shard.log_split + rb), units = ctx->shard.local_units(1ull << log_l) << rb, n_leaves = units * nb;
   o.cols.clear();
   for (const NatSpan& sp : spans)
     for (u32 i = 0; i < sp.cnt; i++) o.cols.push_back(sp.p + (size_t)i * n);
@@ -152,7 +155,7 @@ static int32_t oracle_build_by_coset(bj_ctx* ctx, Oracle& o, const std::vector<N
     for (u64 k = 0; k < units; k++) {
       size_t c0 = 0;
       for (const NatSpan& sp : spans) {
-        BJ_TRY(lde_unit(ctx, sp.p, (uint64_t*)ev.p + c0 * nb, log_n, log_l, sp.cnt, k, 0));
+        BJ_TRY(lde_unit(ctx, sp.p, (uint64_t*)ev.p + c0 * nb, log_n, log_l, sp.cnt, k, 0, rb));
         c0 += sp.cnt;
       }
       // the leaf phase alone: a tree of nb leaves whose cap is its leaves
@@ -342,7 +345,10 @@ struct QueryAnswer {
 // time (oracle_build_by_coset), the quotient runs the streamed plan's unit loop with no kept unit, the openings rebuild coset
 // 0 and DEEP and the queries cosets [0, L), all from the natural-order columns a chunk at a time.  On a sharded context
 // (opt-in of its own) every rank does the same on its own units: its committed units for the trees, DEEP and the queries it
-// answers, its local slot 0 for the openings, its quotient units for the quotient.  The plan replays the
+// answers, its local slot 0 for the openings, its quotient units for the quotient.  On one GPU the recompute plan may cut
+// every coset into B = 2^rb row blocks (bj_ctx_set_max_row_blocks): the trees and the quotient then walk the L * B and Q * B
+// row-block units the way a split shard walks its own, so their scratch is a row block of every column instead of a coset;
+// the openings, DEEP and the queries rebuild whole cosets a chunk of columns at a time as before.  The plan replays the
 // driver's stream-ordered pool allocations in order (pool_peak) and adds what the library keeps outside the pool
 // (library_reserve): twiddles, coset-power tables and the NTT scratch.
 enum MemoryPlan : u32 {
@@ -353,6 +359,7 @@ enum MemoryPlan : u32 {
 };
 struct ProofShape {
   u32 V, C, T, W, n_s2, Q, L, log_n, log_l, log_d, log_q, world, split, cap, n_queries, sched_len;
+  u32 rb = 0;  // one GPU, recompute plan: log2 of the row blocks per coset its trees and quotient are built in
   u32 sched[32];
   u64 n;
   bool lk;
@@ -407,10 +414,11 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk, u64* setup
     m.add(4 * leaves);
     m.add(4 * (leaves - capl));
   };
+  const u64 unit_rows = n >> (s.split + s.rb);  // rows of a tree or quotient unit on the recompute plan
   auto tree_by_coset = [&](u64 cols) {  // oracle_build_by_coset: leaf hashes, one unit of the columns, then the nodes
     m.add(4 * leaves);
-    m.add(cols * (n >> s.split));
-    m.sub(cols * (n >> s.split));
+    m.add(cols * unit_rows);
+    m.sub(cols * unit_rows);
     m.add(4 * (leaves - capl));
   };
   auto rebuild_chunks = [&]() {  // for_chunks: the monomials and one unit (a coset, or a row block) of a chunk of natural columns
@@ -491,8 +499,8 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk, u64* setup
   m.add(2 * nQ);
   const u64 nQl = ((u64)s.Q << s.split) >= w ? nQ / w : n >> s.split;
   if (w > 1) m.add(2 * std::max<u64>(nQl, 1));
-  if (streamed || recompute) {  // one unit of every column the quotient reads (and of z(omega x) on a split shard)
-    const u64 unit = (u64)(s.nat_cols() + (s.split ? 2 : 0)) * (n >> s.split);
+  if (streamed || recompute) {  // one unit of every column the quotient reads (and of z(omega x) on a row block)
+    const u64 unit = (u64)(s.nat_cols() + (s.split + s.rb ? 2 : 0)) * unit_rows;
     m.add(unit);
     m.sub(unit);
   }
@@ -567,6 +575,9 @@ static u64 library_reserve(const ProofShape& s) { return library_tables(s) + lan
 
 static bool compact_applies(const ProofShape& s) { return s.world == 1 && s.Q < s.L; }
 static bool recompute_applies(const ProofShape& s) { return s.world == 1; }
+// one GPU, recompute plan: 1, 2, 4 or 8 row blocks per coset of at least 2 rows each
+static constexpr u32 MAX_LOG_ROW_BLOCKS = 3;
+static bool row_blocks_valid(const ProofShape& s, u32 rb) { return rb <= MAX_LOG_ROW_BLOCKS && s.log_n > rb; }
 // the recompute plan on `world` ranks: the shapes a sharded context takes (at most 8 row blocks per coset, at least 2 rows each)
 static bool sharded_shape_valid(const ProofShape& s) { return s.world <= 8 * s.L && s.log_n > s.split; }
 // ... where every rank owns a unit of the quotient's cosets [0, Q) (with Q < L and more ranks than Q units some own none;
@@ -605,6 +616,7 @@ struct bj_setup {
   bool compact = false;   // memory plan chosen by bj_setup_create, followed by bj_prove
   bool streamed = false;
   bool recompute = false;
+  uint32_t log_blocks = 0;  // recompute plan on one GPU: log2 of the row blocks per coset (bj_setup_row_blocks), 0 elsewhere
   uint64_t limit = 0;    // the device-memory limit the plan was chosen under
   uint64_t plan[4] = {0, 0, 0, 0};  // resident, compact, streamed, recompute (0: the plan does not apply or was not allowed)
   uint32_t chunk = 2;         // compact and recompute plans: natural-order columns recomputed at a time
@@ -749,18 +761,34 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
     s->plan[2] = streamed_applies(sh) ? plan_bytes(sh, PLAN_STREAMED) : 0;
     const bool recompute_allowed = (ctx->allow_recompute_plan && recompute_applies(sh)) ||
                                    (ctx->allow_sharded_recompute_plan && ctx->comm && recompute_sharded_applies(sh));
-    s->plan[3] = recompute_allowed ? plan_bytes(sh, PLAN_RECOMPUTE) : 0;
     BJ_TRY(memory_limit(ctx, &s->limit));
     // with lanes alive on the context, a plan must also hold their proofs: one lane part each beside the plan
     const uint32_t lanes = ctx->lanes.load();
-    uint64_t need[4];
-    for (int k = 0; k < 4; k++) {
-      need[k] = s->plan[k];
-      if (need[k] && lanes) {
+    auto need_of = [&](const ProofShape& shape, MemoryPlan k) {
+      uint64_t v = plan_bytes(shape, k);
+      if (lanes) {
         uint64_t lp[3];
-        lane_plan(sh, (MemoryPlan)k, 2, 1, lp);
-        need[k] += (uint64_t)lanes * lp[1];
+        lane_plan(shape, k, 2, 1, lp);
+        v += (uint64_t)lanes * lp[1];
       }
+      return v;
+    };
+    uint64_t need[4];
+    for (int k = 0; k < 3; k++) need[k] = s->plan[k] ? need_of(sh, (MemoryPlan)k) : 0;
+    // the recompute plan on one GPU: the fewest row blocks per coset (up to the context's bj_ctx_set_max_row_blocks) whose
+    // plan fits, or the most allowed when none does, so that a refusal names the smallest recompute plan on offer
+    uint32_t rb = 0;
+    need[3] = 0;
+    if (recompute_allowed) {
+      uint32_t max_rb = 0;
+      while (!ctx->comm && (2u << max_rb) <= ctx->max_row_blocks && row_blocks_valid(sh, max_rb + 1)) max_rb++;
+      ProofShape shb = sh;
+      for (;; rb++) {
+        shb.rb = rb;
+        need[3] = need_of(shb, PLAN_RECOMPUTE);
+        if (need[3] <= s->limit || rb == max_rb) break;
+      }
+      s->plan[3] = plan_bytes(shb, PLAN_RECOMPUTE);
     }
     auto fits = [&](int k) { return need[k] && need[k] <= s->limit; };
     if (need[0] > s->limit) {
@@ -794,6 +822,8 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
         s->recompute = true;
       }
     }
+    if (s->recompute) s->log_blocks = rb;
+    sh.rb = s->log_blocks;
     if (s->compact || s->recompute) {
       // wider recompute chunks only save kernel launches: the chunk grows into at most half of the headroom the limit leaves
       // over the plan (the rest is slack for the pool's fragmentation) and stops at 16 columns
@@ -851,7 +881,7 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
   // tree is built one coset at a time, and s->tree.cols are the natural-order columns every reader rebuilds its cosets from.
   if (s->recompute) {
     BJ_TRY(oracle_build_by_coset(ctx, s->tree, {{d_sigmas, V}, {d_constants, C}, {d_lookup_tables, T}}, log_n, log_l,
-                                 circuit->merkle_tree_cap_size, circuit->tree_hasher));
+                                 circuit->merkle_tree_cap_size, circuit->tree_hasher, s->log_blocks));
     return publish();
   }
   const uint32_t log_kept = s->streamed ? log_l : log_d;
@@ -916,6 +946,7 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   const uint32_t split = ctx->shard.log_split;                            // 2^split row blocks per coset (split domain shard)
   const u64 nb = n >> split;                                             // rows of one unit
   const bool compact = setup->compact, streamed = setup->streamed, recompute = setup->recompute;
+  const uint32_t rb = setup->log_blocks;  // recompute plan on one GPU: 2^rb row blocks per coset in the trees and the quotient
   const u64 Qn = n * Q;  // compact plan: elements of a setup / witness / stage-2 column kept on the device (cosets [0, Q))
   const uint32_t log_kept = streamed ? log_l : log_d;  // streamed plan: those columns are evaluated on the cosets [0, L) only
   const u64 nK = streamed ? nL : nD;      // stride of those columns on the resident and streamed plans
@@ -974,7 +1005,7 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   const uint64_t* m_col = nullptr;
   Oracle w_or;
   if (recompute) {  // the tree one coset at a time; the columns stand for themselves in natural order from here on
-    BJ_TRY(oracle_build_by_coset(ctx, w_or, {{d_variables, V}, {d_multiplicities, lk ? 1u : 0u}}, log_n, log_l, cap, c.tree_hasher));
+    BJ_TRY(oracle_build_by_coset(ctx, w_or, {{d_variables, V}, {d_multiplicities, lk ? 1u : 0u}}, log_n, log_l, cap, c.tree_hasher, rb));
     for (uint32_t j = 0; j < V; j++) w_cols[j] = w_or.cols[j];
     if (lk) m_col = w_or.cols[V];
   } else if (compact) {
@@ -1042,7 +1073,7 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
   std::vector<const uint64_t*> s2_cols(n_s2);
   Oracle s2_or;
   if (recompute) {
-    BJ_TRY(oracle_build_by_coset(ctx, s2_or, {{(const uint64_t*)st2.p, n_s2}}, log_n, log_l, cap, c.tree_hasher));
+    BJ_TRY(oracle_build_by_coset(ctx, s2_or, {{(const uint64_t*)st2.p, n_s2}}, log_n, log_l, cap, c.tree_hasher, rb));
     s2_cols = s2_or.cols;
   } else if (compact) {
     BJ_TRY(lde_grouped(ctx, s2_groups, (const uint64_t*)st2.p, n_s2, log_n, log_d, s2_cols.data()));
@@ -1132,7 +1163,7 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
       std::vector<uint64_t> nr(V);
       BJ_TRY(bj_non_residues_for_copy_permutation(n, V, nr.data()));
       const uint64_t b[2] = {beta.c0, beta.c1}, g[2] = {gamma.c0, gamma.c1};
-      if (split)
+      if (ctx->shard.log_split)  // a row block (split shard, or a recompute unit under its window) does not hold z(omega x)
         BJ_TRY(bj_quotient_copy_permutation_with_z_next(ctx, k.w.data(), k.sigma.data(), V, nr.data(), k.s2[0], k.s2[1], k.z_next0,
                                                         k.z_next1, n_partial ? k.s2.data() + 2 : nullptr, b, g,
                                                         powers.data() + 2 * (size_t)(n_lk_terms + n_gate_terms), log_n, log_d, log_q, Q, o0, o1));
@@ -1147,17 +1178,21 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     const uint64_t* zn = (const uint64_t*)z_next.p;
     if (nQl) BJ_TRY(quotient_terms({w_cols, sigma_cols, const_cols, table_cols, s2_cols, m_col, zn, zn ? zn + nD : nullptr}, nQl, q0, q1));
   } else {
-    // one local quotient unit k at a time (global unit u: coset u on one GPU or a coset shard, a row block of nb rows of
-    // coset u / B on a split shard), under the window of unit u among the units of the factor-D domain.  On the streamed
-    // plan the units of the committed cosets [0, L) come from the kept columns (their first L * B / world local units); the
-    // others, and every unit on the recompute plan, are evaluated into one unit-sized scratch from the natural-order
-    // columns; on a split shard the unit's z(omega x) columns go to the scratch too.
-    const CosetShard shard = ctx->shard;
+    // one local quotient unit k at a time (global unit u: coset u on one GPU or a coset shard, a row block of ub rows of
+    // coset u / B on a split shard or on one GPU with 2^rb row blocks per coset), under the window of unit u among the units
+    // of the factor-D domain.  On the streamed plan the units of the committed cosets [0, L) come from the kept columns
+    // (their first L * B / world local units); the others, and every unit on the recompute plan, are evaluated into one
+    // unit-sized scratch from the natural-order columns; on a row block the unit's z(omega x) columns go to the scratch too.
+    // The unit's quotient values land in its slot [k ub, (k + 1) ub) of the local quotient cosets.
+    CosetShard shard = ctx->shard;
+    shard.log_split += rb;  // one GPU: every one of the Q * 2^rb units is local, global unit k = k
+    const uint32_t usplit = shard.log_split;
+    const u64 ub = n >> usplit;
     const u64 q_units = shard.local_units(Q), kept_units = recompute ? 0 : shard.local_units(L);
     DevMem ev;
-    BJ_TRY(ev.alloc(ctx, (size_t)(2 * V + C + T + (lk ? 1 : 0) + n_s2 + (split ? 2 : 0)) * nb));
+    BJ_TRY(ev.alloc(ctx, (size_t)(2 * V + C + T + (lk ? 1 : 0) + n_s2 + (usplit ? 2 : 0)) * ub));
     for (u64 k = 0; k < q_units; k++) {
-      ShardWindow window(ctx, log_d + split, (u32)shard.global_unit(k), split);
+      ShardWindow window(ctx, log_d + usplit, (u32)shard.global_unit(k), usplit);
       QuotientCols qc;
       uint64_t* e = (uint64_t*)ev.p;
       // columns `kept` moved to unit k, or `cnt` natural columns of `nat` evaluated on unit u into the next slots of ev
@@ -1165,12 +1200,12 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
       auto unit_k = [&](const std::vector<const uint64_t*>& kept_cols, const uint64_t* nat, uint32_t cnt, std::vector<const uint64_t*>& out) -> int32_t {
         out.resize(cnt);
         if (k < kept_units) {
-          for (uint32_t i = 0; i < cnt; i++) out[i] = kept_cols[i] + (size_t)k * nb;
+          for (uint32_t i = 0; i < cnt; i++) out[i] = kept_cols[i] + (size_t)k * ub;
           return BJ_OK;
         }
         if (cnt) BJ_TRY(bj_lde(ctx, nat, n, e, log_n, log_d, cnt, 0));
-        for (uint32_t i = 0; i < cnt; i++) out[i] = e + (size_t)i * nb;
-        e += (size_t)cnt * nb;
+        for (uint32_t i = 0; i < cnt; i++) out[i] = e + (size_t)i * ub;
+        e += (size_t)cnt * ub;
         return BJ_OK;
       };
       BJ_TRY(unit_k(w_cols, d_variables, V, qc.w));
@@ -1182,12 +1217,12 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
       if (lk) BJ_TRY(unit_k({m_col}, d_multiplicities, 1, mj));
       qc.m = lk ? mj[0] : nullptr;
       qc.z_next0 = qc.z_next1 = nullptr;
-      if (split) {
+      if (usplit) {
         BJ_TRY(bj_lde_next_row(ctx, (const uint64_t*)st2.p, n, e, log_n, log_d, 2, 0));
         qc.z_next0 = e;
-        qc.z_next1 = e + nb;
+        qc.z_next1 = e + ub;
       }
-      BJ_TRY(quotient_terms(qc, nb, q0 + (size_t)k * nb, q1 + (size_t)k * nb));
+      BJ_TRY(quotient_terms(qc, ub, q0 + (size_t)k * ub, q1 + (size_t)k * ub));
     }
   }
   z_next.release();
@@ -1801,10 +1836,29 @@ int32_t bj_proof_memory_plan_recompute_sharded(const bj_circuit* circuit, uint32
   return BJ_OK;
 }
 
-int32_t bj_proof_memory_plan_lanes_host(const bj_circuit* circuit, uint32_t plan, uint32_t n_lanes, uint64_t out[3]) {
+// log2 of a row-block count of the one-GPU recompute plan: 1, 2, 4 or 8 row blocks of at least 2 rows each
+static int32_t log_row_blocks(const ProofShape& sh, uint32_t blocks, uint32_t* rb) {
+  if (!is_pow2(blocks)) return BJ_ERR_INVALID_ARG;
+  *rb = 0;
+  while ((1u << *rb) < blocks) (*rb)++;
+  return row_blocks_valid(sh, *rb) ? BJ_OK : BJ_ERR_INVALID_ARG;
+}
+
+int32_t bj_proof_memory_plan_recompute_blocks(const bj_circuit* circuit, uint32_t blocks, uint64_t* out) {
   ProofShape sh;
-  if (!out || n_lanes == 0 || plan > BJ_PLAN_RECOMPUTE) return BJ_ERR_INVALID_ARG;
+  if (!out) return BJ_ERR_INVALID_ARG;
+  *out = 0;
   BJ_TRY(memory_plan_shape(circuit, 1, &sh));
+  BJ_TRY(log_row_blocks(sh, blocks, &sh.rb));
+  *out = plan_bytes(sh, PLAN_RECOMPUTE);
+  return BJ_OK;
+}
+
+int32_t bj_proof_memory_plan_lanes_host_blocks(const bj_circuit* circuit, uint32_t plan, uint32_t blocks, uint32_t n_lanes, uint64_t out[3]) {
+  ProofShape sh;
+  if (!out || n_lanes == 0 || plan > BJ_PLAN_RECOMPUTE || (plan != BJ_PLAN_RECOMPUTE && blocks != 1)) return BJ_ERR_INVALID_ARG;
+  BJ_TRY(memory_plan_shape(circuit, 1, &sh));
+  BJ_TRY(log_row_blocks(sh, blocks, &sh.rb));
   const bool applies = plan == PLAN_RESIDENT || (plan == PLAN_COMPACT && compact_applies(sh)) || (plan == PLAN_STREAMED && streamed_applies(sh)) ||
                        (plan == PLAN_RECOMPUTE && recompute_applies(sh));
   if (!applies) {
@@ -1815,6 +1869,17 @@ int32_t bj_proof_memory_plan_lanes_host(const bj_circuit* circuit, uint32_t plan
   return BJ_OK;
 }
 
+int32_t bj_proof_memory_plan_lanes_host(const bj_circuit* circuit, uint32_t plan, uint32_t n_lanes, uint64_t out[3]) {
+  return bj_proof_memory_plan_lanes_host_blocks(circuit, plan, 1, n_lanes, out);
+}
+
+// the one-GPU shape of a setup's chosen plan, row blocks included
+static int32_t setup_shape(const bj_setup* s, ProofShape* sh) {
+  BJ_TRY(proof_shape(s->c, 1, sh));
+  sh->rb = s->log_blocks;
+  return BJ_OK;
+}
+
 static MemoryPlan setup_plan_kind(const bj_setup* s) {
   return s->compact ? PLAN_COMPACT : s->streamed ? PLAN_STREAMED : s->recompute ? PLAN_RECOMPUTE : PLAN_RESIDENT;
 }
@@ -1822,7 +1887,7 @@ static MemoryPlan setup_plan_kind(const bj_setup* s) {
 int32_t bj_proof_memory_plan_lanes(const bj_setup* setup, uint32_t n_lanes, uint64_t out[3]) {
   ProofShape sh;
   if (!setup || !out || n_lanes == 0 || comm_world(setup->ctx) != 1) return BJ_ERR_INVALID_ARG;
-  BJ_TRY(proof_shape(setup->c, 1, &sh));
+  BJ_TRY(setup_shape(setup, &sh));
   lane_plan(sh, setup_plan_kind(setup), setup->chunk, n_lanes, out);
   return BJ_OK;
 }
@@ -1830,7 +1895,7 @@ int32_t bj_proof_memory_plan_lanes(const bj_setup* setup, uint32_t n_lanes, uint
 int32_t bj_proof_memory_plan_lane_pool(const bj_setup* setup, uint64_t* pool_bytes) {
   ProofShape sh;
   if (!setup || !pool_bytes || comm_world(setup->ctx) != 1) return BJ_ERR_INVALID_ARG;
-  BJ_TRY(proof_shape(setup->c, 1, &sh));
+  BJ_TRY(setup_shape(setup, &sh));
   uint64_t out[3];
   lane_plan(sh, setup_plan_kind(setup), setup->chunk, 1, out);
   *pool_bytes = out[1] - lane_reserve(sh);
@@ -1852,7 +1917,7 @@ int32_t bj_ctx_create_lane(bj_ctx* parent, bj_ctx** out) {
     const uint32_t lanes_after = parent->lanes.load() + 1;
     for (const bj_setup* s : parent->setups) {
       ProofShape sh;
-      BJ_TRY(proof_shape(s->c, 1, &sh));
+      BJ_TRY(setup_shape(s, &sh));
       uint64_t p[3];
       lane_plan(sh, setup_plan_kind(s), s->chunk, lanes_after + 1, p);
       const uint64_t limit = parent->memory_limit ? parent->memory_limit : s->limit;
@@ -1871,6 +1936,8 @@ int32_t bj_setup_plan(const bj_setup* s) {
   if (!s) return BJ_ERR_INVALID_ARG;
   return s->compact ? BJ_PLAN_COMPACT : s->streamed ? BJ_PLAN_STREAMED : s->recompute ? BJ_PLAN_RECOMPUTE : BJ_PLAN_RESIDENT;
 }
+
+int32_t bj_setup_row_blocks(const bj_setup* s) { return s ? (int32_t)(1u << s->log_blocks) : BJ_ERR_INVALID_ARG; }
 
 int32_t bj_setup_memory_plan(const bj_setup* s, uint64_t out[3]) {
   if (!s || !out) return BJ_ERR_INVALID_ARG;

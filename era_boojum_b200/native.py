@@ -52,6 +52,7 @@ SIGNATURES = {
     "bj_ctx_set_memory_limit": (_i32, [_vp, _u64]),
     "bj_ctx_allow_recompute_plan": (_i32, [_vp, _i32]),
     "bj_ctx_allow_sharded_recompute_plan": (_i32, [_vp, _i32]),
+    "bj_ctx_set_max_row_blocks": (_i32, [_vp, _u32]),
     "bj_ctx_memory_high_water": (_i32, [_vp, _vp, _i32]),
     "bj_ctx_create_lane": (_i32, [_vp, _pp]),
     "bj_alloc": (_i32, [_vp, _sz, _pp]),
@@ -133,12 +134,15 @@ SIGNATURES = {
     "bj_proof_memory_plan_streamed_sharded": (_i32, [_vp, _u32, _vp]),
     "bj_proof_memory_plan_recompute": (_i32, [_vp, _u32, _vp]),
     "bj_proof_memory_plan_recompute_sharded": (_i32, [_vp, _u32, _vp]),
+    "bj_proof_memory_plan_recompute_blocks": (_i32, [_vp, _u32, _vp]),
     "bj_setup_is_compact": (_i32, [_vp]),
     "bj_setup_plan": (_i32, [_vp]),
+    "bj_setup_row_blocks": (_i32, [_vp]),
     "bj_setup_memory_plan": (_i32, [_vp, _vp]),
     "bj_proof_memory_plan_lanes": (_i32, [_vp, _u32, _vp]),
     "bj_proof_memory_plan_lane_pool": (_i32, [_vp, _vp]),
     "bj_proof_memory_plan_lanes_host": (_i32, [_vp, _u32, _u32, _vp]),
+    "bj_proof_memory_plan_lanes_host_blocks": (_i32, [_vp, _u32, _u32, _u32, _vp]),
     "bj_setup_get_cap": (_i32, [_vp, _vp]),
     "bj_prove": (_i32, [_vp, _vp, _vp, _vp, _pp]),
     "bj_proof_free": (None, [_vp]),

@@ -92,6 +92,14 @@ BJ_API int32_t bj_ctx_set_memory_limit(bj_ctx* ctx, uint64_t bytes);
  * the recompute plan rebuilds every coset of the setup, witness and stage-2 columns wherever it is read, so it is slower, and
  * a caller that relies on BJ_ERR_OOM below the smaller plans keeps it.  A sharded context ignores the switch. */
 BJ_API int32_t bj_ctx_allow_recompute_plan(bj_ctx* ctx, int32_t allow);
+/* Row blocks per coset the one-GPU RECOMPUTE plan may use: max_blocks = 1 (the default), 2, 4 or 8, anything else
+ * BJ_ERR_INVALID_ARG.  When bj_setup_create takes the recompute plan (still only after bj_ctx_allow_recompute_plan) it takes
+ * the fewest row blocks B <= max_blocks whose plan (bj_proof_memory_plan_recompute_blocks) fits under the limit; the refusal
+ * below every plan names the recompute bytes at the largest allowed B.  With B > 1 the trees and the quotient work on the
+ * L * B and Q * B row blocks of n / B rows (B >= 2 rows each) instead of whole cosets, so their scratch falls by B while the
+ * quotient repeats the inverse NTT of its columns B times as often; every other choice, refusal and proof is unchanged.
+ * bj_setup_row_blocks reports the B chosen.  A context with a communicator ignores the switch; lanes inherit it. */
+BJ_API int32_t bj_ctx_set_max_row_blocks(bj_ctx* ctx, uint32_t max_blocks);
 /* allow != 0 lets bj_setup_create on a context with a communicator fall back to the RECOMPUTE plan on this rank
  * (bj_proof_memory_plan_recompute_sharded) when neither RESIDENT nor STREAMED fits under the rank's limit; the refusal below
  * every plan then names the recompute bytes too.  Off by default, for the reasons of bj_ctx_allow_recompute_plan, which a
@@ -562,6 +570,14 @@ BJ_API int32_t bj_proof_memory_plan_recompute(const bj_circuit* circuit, uint32_
  * shapes sharding rejects: cap_size < world, world > 8 * LDE factor, a row block of fewer than 2 rows.  Chosen only after
  * bj_ctx_allow_sharded_recompute_plan. */
 BJ_API int32_t bj_proof_memory_plan_recompute_sharded(const bj_circuit* circuit, uint32_t world, uint64_t* out);
+/* The one-GPU RECOMPUTE plan's bytes with every coset cut into `blocks` row blocks (host only, no device needed): each tree is
+ * built one row block of n / blocks rows at a time (its columns evaluated from natural order into a row-block scratch per
+ * column, its leaves hashed into their slice) and the quotient evaluates every column it reads, and z(omega x), onto one of
+ * the Q * blocks row blocks of cosets [0, Q) at a time.  The openings, DEEP and the query answers rebuild whole cosets as on
+ * the recompute plan.  At blocks = 1 the value of bj_proof_memory_plan_recompute(circuit, 1, out).  *out = 0 and
+ * BJ_ERR_INVALID_ARG for blocks other than 1, 2, 4 or 8, or row blocks of fewer than 2 rows.  Proofs are bit-identical to
+ * the resident plan's; chosen only after bj_ctx_allow_recompute_plan and bj_ctx_set_max_row_blocks. */
+BJ_API int32_t bj_proof_memory_plan_recompute_blocks(const bj_circuit* circuit, uint32_t blocks, uint64_t* out);
 /* 1 if bj_setup_create chose the compact plan, 0 otherwise (resident, streamed or recompute) */
 BJ_API int32_t bj_setup_is_compact(const bj_setup* setup);
 /* the plan bj_setup_create chose: BJ_PLAN_RESIDENT, BJ_PLAN_COMPACT, BJ_PLAN_STREAMED or BJ_PLAN_RECOMPUTE */
@@ -570,6 +586,9 @@ BJ_API int32_t bj_setup_is_compact(const bj_setup* setup);
 #define BJ_PLAN_STREAMED 2
 #define BJ_PLAN_RECOMPUTE 3
 BJ_API int32_t bj_setup_plan(const bj_setup* setup);
+/* the row blocks per coset bj_setup_create chose for the recompute plan on one GPU (bj_ctx_set_max_row_blocks); 1 on every
+ * other plan and on a sharded context */
+BJ_API int32_t bj_setup_row_blocks(const bj_setup* setup);
 /* the plan bj_setup_create chose: out[0] the peak bytes of the context's pool over bj_setup_create + bj_prove (what
  * bj_ctx_memory_high_water reads on a fresh context), out[1] the bound on what the library holds outside the pool, out[2] the
  * columns the compact or recompute plan recomputes at a time (0 on the resident and streamed plans) */
@@ -587,6 +606,11 @@ BJ_API int32_t bj_proof_memory_plan_lane_pool(const bj_setup* setup, uint64_t* p
  * with the smallest recompute chunk: out[0] + out[1] equals bj_proof_memory_plan(_streamed / _recompute) for that plan; all
  * three are 0 where the plan does not apply to the circuit */
 BJ_API int32_t bj_proof_memory_plan_lanes_host(const bj_circuit* circuit, uint32_t plan, uint32_t n_lanes, uint64_t out[3]);
+/* bj_proof_memory_plan_lanes_host with the recompute plan cut into `blocks` row blocks per coset (1, 2, 4 or 8; only 1 on the
+ * other plans, else BJ_ERR_INVALID_ARG): out[0] + out[1] equals bj_proof_memory_plan_recompute_blocks.  bj_proof_memory_plan_lanes
+ * and bj_witness_slots_create count the row blocks a setup chose by themselves. */
+BJ_API int32_t bj_proof_memory_plan_lanes_host_blocks(const bj_circuit* circuit, uint32_t plan, uint32_t blocks, uint32_t n_lanes,
+                                                      uint64_t out[3]);
 BJ_API int32_t bj_setup_get_cap(const bj_setup* setup, uint64_t* h_cap /* 4 * cap_size u64: VerificationKey::setup_merkle_tree_cap */);
 BJ_API int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables, const uint64_t* d_multiplicities /* or NULL */,
                  bj_proof** out);
