@@ -801,6 +801,19 @@ def witness_slots_bytes(log_n, num_variables, n_slots, max_values=0, lookup=None
     return int(out.value)
 
 
+def witness_slots_bytes_split(log_n, num_variables, n_slots, max_values=0, lookup=None):
+    """bj_witness_slots_bytes_split: witness_slots_bytes at world 1 split in two -> (bytes the set itself allocates in its
+    context's pool, bytes of the u32 variables hint, which lives once on the setup: 0 when max_values == 0).  A set on a lane
+    (NativeSetup.witness_slots(..., ctx=lane)) counts the first only (no device needed)"""
+    c = native.Circuit()
+    c.log_n, c.num_variables = log_n, num_variables
+    if lookup:
+        c.lookup_width, c.lookup_num_repetitions = lookup["width"], lookup["num_repetitions"]
+    out = (ctypes.c_uint64 * 2)()
+    _ok(lib.bj_witness_slots_bytes_split(ctypes.byref(c), n_slots, max_values, out), "bj_witness_slots_bytes_split")
+    return int(out[0]), int(out[1])
+
+
 def variables_hint_to_u32(hint):
     """bj_variables_hint_to_u32: reference `Variable`s (bit 63 = placeholder) -> (u32 hint with placeholders 0xFFFFFFFF, 1 + the
     largest index).  Raises BoojumError(BJ_ERR_INVALID_ARG) on an index >= 2^32 - 1."""
@@ -810,6 +823,11 @@ def variables_hint_to_u32(hint):
     _ok(lib.bj_variables_hint_to_u32(h.ctypes.data_as(ctypes.c_void_p), h.size, out.ctypes.data_as(ctypes.c_void_p), ctypes.byref(need)),
         "bj_variables_hint_to_u32")
     return out, int(need.value)
+
+
+def _on_device(witness):
+    """True for a witness of CUDA tensors, False for host arrays"""
+    return bool(getattr(witness[0], "is_cuda", False))
 
 
 def _host_array(a, dtype, n):
@@ -825,10 +843,11 @@ def _host_array(a, dtype, n):
 
 class WitnessSlots:
     """bj_witness_slots: witness slots of one NativeSetup on the device, filled from host memory on the context's copy stream
-    while proofs run on its stream."""
+    while proofs run on its stream.  ctx: the setup's context (the default) or one of its lanes (Context.lane), whose own copy
+    stream, pool and stream the set then uses; only that lane's thread may use the set."""
 
-    def __init__(self, setup, n, max_values=0):
-        self.setup, self.ctx, self.n, self.max_values = setup, setup.ctx, n, max_values
+    def __init__(self, setup, n, max_values=0, ctx=None):
+        self.setup, self.ctx, self.n, self.max_values = setup, ctx or setup.ctx, n, max_values
         _, self.V, _, _, _, _, lookup, _ = setup._vk_args
         self.lookup = bool(lookup)
         self.rows = 1 << setup._vk_args[0]
@@ -990,11 +1009,12 @@ class NativeSetup:
 
     has_hint = False
 
-    def witness_slots(self, n=2, max_values=0):
+    def witness_slots(self, n=2, max_values=0, ctx=None):
         """bj_witness_slots_create: n (1 to 4) device slots for witnesses of this setup, plus a WitnessVec buffer of max_values
-        values when max_values > 0"""
-        ws = WitnessSlots(self, n, max_values)
-        self.ctx._children.add(ws)
+        values when max_values > 0.  ctx: this setup's context (the default) or one of its lanes; prove_stream(..., slots=set)
+        then proves on that lane.  Attach the hint before creating sets on lanes."""
+        ws = WitnessSlots(self, n, max_values, ctx)
+        ws.ctx._children.add(ws)
         return ws
 
     def prove_stream(self, witnesses, as_json=True, slots=None):
@@ -1027,12 +1047,39 @@ class NativeSetup:
             if own:
                 slots.close()
 
-    def prove_concurrent(self, witnesses, lanes=2, as_json=True):
+    def prove_concurrent(self, witnesses, lanes=2, as_json=True, slots_per_lane=2):
         """Proves several witnesses at once on this setup's GPU, yielding the proofs in input order (each the bytes
-        prove() returns).  witnesses: an iterable of (variables [V, n], multiplicities [n] or None) CUDA tensors, complete
-        on the current torch stream when they are taken from the iterable.  `lanes` lane contexts (Context.lane) prove
-        them from a thread pool, at most two witnesses per lane ahead of the one yielded; the lanes are closed at the end.
-        Lanes do not combine with witness slots or prove_stream: those run on the setup's own context."""
+        prove() returns).  `lanes` lane contexts (Context.lane) prove them, each from its own thread; the lanes are closed at
+        the end, also on an exception.  witnesses: an iterable of
+          - (variables [V, n], multiplicities [n] or None) CUDA tensors, complete on the current torch stream when they are
+            taken from the iterable, proved from a thread pool, at most two witnesses per lane ahead of the one yielded; or
+          - host witnesses: the host arrays prove_stream takes (numpy or CPU torch, pinned or pageable; WitnessVec pairs once
+            a hint is attached).  Witness i goes to lane i % lanes, which runs prove_stream over its share through its own
+            slot set of `slots_per_lane` slots (uploads on the lane's copy stream overlap its proofs), at most
+            lanes * slots_per_lane witnesses ahead of the one yielded.  The slot sets are freed at the end.
+        A mix of device and host witnesses raises ValueError: for a list or tuple before any proof, for another iterable when
+        the first witness of the other kind is taken."""
+        if isinstance(witnesses, (list, tuple)) and len({_on_device(w) for w in witnesses}) > 1:
+            raise ValueError("prove_concurrent: the witnesses mix CUDA tensors and host arrays")
+        it = iter(witnesses)
+        try:
+            first = next(it)
+        except StopIteration:
+            return
+        device = _on_device(first)
+
+        def checked():
+            for w in itertools.chain([first], it):
+                if _on_device(w) != device:
+                    raise ValueError("prove_concurrent: the witnesses mix CUDA tensors and host arrays")
+                yield w
+
+        if device:
+            yield from self._prove_concurrent_device(checked(), lanes, as_json)
+        else:
+            yield from self._prove_concurrent_host(checked(), len(first[0]) if self.has_hint else 0, lanes, as_json, slots_per_lane)
+
+    def _prove_concurrent_device(self, witnesses, lanes, as_json):
         import collections
         import queue
         from concurrent.futures import ThreadPoolExecutor
@@ -1061,6 +1108,67 @@ class NativeSetup:
                 yield pending.popleft().result()
         finally:
             pool.shutdown(wait=True, cancel_futures=True)
+            for c in ctxs:
+                c.close()
+
+    def _prove_concurrent_host(self, witnesses, max_values, lanes, as_json, slots_per_lane):
+        import queue
+        import threading
+        end = object()
+        stop = threading.Event()
+        inbox = [queue.Queue() for _ in range(lanes)]
+        outbox = [queue.Queue() for _ in range(lanes)]
+        ctxs, sets, threads = [], [], []
+
+        def lane_main(k):
+            def feed():
+                while not stop.is_set():
+                    w = inbox[k].get()
+                    if w is end:
+                        return
+                    yield w
+            try:
+                for p in self.prove_stream(feed(), as_json=as_json, slots=sets[k]):
+                    outbox[k].put((True, p))
+            except BaseException as e:  # noqa: BLE001 - raised on the caller's thread
+                outbox[k].put((False, e))
+
+        def result(i):
+            ok, v = outbox[i % lanes].get()
+            if not ok:
+                raise v
+            return v
+
+        try:
+            for _ in range(lanes):
+                ctxs.append(self.ctx.lane())
+                sets.append(self.witness_slots(slots_per_lane, max_values, ctx=ctxs[-1]))
+            threads = [threading.Thread(target=lane_main, args=(k,), daemon=True) for k in range(lanes)]
+            for t in threads:
+                t.start()
+            # a lane yields witness i's proof once it holds slots_per_lane - 1 later witnesses (or the end): those are
+            # queued before the proof is awaited
+            ahead = lanes * slots_per_lane
+            taken = done = 0
+            for w in witnesses:
+                inbox[taken % lanes].put(w)
+                taken += 1
+                if taken - done >= ahead:
+                    yield result(done)
+                    done += 1
+            for q in inbox:
+                q.put(end)
+            while done < taken:
+                yield result(done)
+                done += 1
+        finally:
+            stop.set()
+            for q in inbox:
+                q.put(end)
+            for t in threads:
+                t.join()
+            for ws in sets:
+                ws.close()
             for c in ctxs:
                 c.close()
 

@@ -215,6 +215,11 @@ int32_t bj_ctx_destroy(bj_ctx* ctx) {
   bj::DeviceGuard device_guard(ctx);
   if (const uint32_t alive = ctx->lanes.load())
     BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_ctx_destroy: " + std::to_string(alive) + " lane(s) of this context are alive: destroy them first");
+  if (ctx->parent) {
+    std::lock_guard<std::mutex> lock(ctx->parent->tables_mu);
+    if (ctx->witness_sets)
+      BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_ctx_destroy: " + std::to_string(ctx->witness_sets) + " witness slot set(s) of this lane are alive: free them first");
+  }
   cudaStreamSynchronize(ctx->stream);
   if (ctx->witness_stream) {  // uploads of witness slot sets still in flight finish before the memory goes
     cudaStreamSynchronize(ctx->witness_stream);

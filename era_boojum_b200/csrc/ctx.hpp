@@ -115,8 +115,16 @@ struct bj_ctx {
   cudaEvent_t ev_up[3] = {}, ev_done[3] = {}, ev_down[3] = {};
   void* host_ring = nullptr;
   size_t host_ring_bytes = 0;
-  // witness slot sets (witness_stream.cu): the copy stream their uploads run on, created by the first slot set
+  // witness slot sets (witness_stream.cu): the copy stream their uploads run on, created by the first slot set (a lane's by
+  // its first slot set, destroyed with the lane)
   cudaStream_t witness_stream = nullptr;
+  // slot sets alive on this context and the pool bytes they count: a parent's sets their full bj_witness_slots_bytes, a
+  // lane's sets out[0] of bj_witness_slots_bytes_split.  On a parent, lane_witness_* sums the sets of all its lanes.  A lane's
+  // fields and its parent's lane_witness_* are read and written under the parent's tables_mu.
+  uint32_t witness_sets = 0;
+  uint64_t witness_set_bytes = 0;
+  uint32_t lane_witness_sets = 0;
+  uint64_t lane_witness_set_bytes = 0;
   void* param_arena = nullptr;  // bump arena for small per-call parameter blocks
   size_t param_off = 0;
   uint64_t launches = 0;  // kernels launched by this library through this context
@@ -163,10 +171,15 @@ struct bj_ctx {
   //    not pin (ntt_l2_persist = 0); N streams pinning N tables into one carve-out would only evict one another.
   //  - Poseidon2 round constants: device constant memory written once by bj_ctx_create; a lane does not rewrite them.
   //  - the setups of the parent are read only; bj_prove on a lane first waits for the setup's ready event.
-  // Teardown: bj_ctx_destroy refuses a context with lanes alive; lanes are destroyed first.
+  //  - witness slot sets created on a lane (witness_stream.cu) and the lane's witness_stream: the lane's own, touched by the
+  //    lane's thread only.  Their buffers and pinned staging ring belong to the set and come from the lane's pool; a
+  //    WitnessVec gather on the lane's copy stream reads the setup's u32 hint (the parent's pool), which
+  //    bj_setup_attach_variables_hint refuses to replace while a lane's set is alive.  The counts of live sets (witness_sets,
+  //    the parent's lane_witness_*) are kept under the parent's tables_mu, for the memory checks of the parent's thread.
+  // Teardown: bj_ctx_destroy refuses a context with lanes alive, and a lane with slot sets alive; sets go first, then lanes.
   bj_ctx* parent = nullptr;       // a lane's parent (nullptr: a context of bj_ctx_create)
   std::atomic<uint32_t> lanes{0};  // lanes of this context alive
-  std::mutex tables_mu;            // guards tw_*, pow_cache, pow_full_bytes, tables_retired and setups (see above)
+  std::mutex tables_mu;            // guards tw_*, pow_cache, pow_full_bytes, tables_retired, setups and the set counts (see above)
   std::vector<void*> tables_retired;
   bool own_twiddles = true;        // false while a lane's tw_* view the parent's pair
   std::vector<const bj_setup*> setups;  // setups alive on this context: bj_ctx_create_lane plans against them

@@ -762,14 +762,20 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
     const bool recompute_allowed = (ctx->allow_recompute_plan && recompute_applies(sh)) ||
                                    (ctx->allow_sharded_recompute_plan && ctx->comm && recompute_sharded_applies(sh));
     BJ_TRY(memory_limit(ctx, &s->limit));
-    // with lanes alive on the context, a plan must also hold their proofs: one lane part each beside the plan
+    // with lanes alive on the context, a plan must also hold their proofs: one lane part each beside the plan, and the
+    // witness slot sets alive on the lanes
     const uint32_t lanes = ctx->lanes.load();
+    uint64_t lane_sets = 0;
+    {
+      std::lock_guard<std::mutex> lock(ctx->tables_mu);
+      lane_sets = ctx->lane_witness_set_bytes;
+    }
     auto need_of = [&](const ProofShape& shape, MemoryPlan k) {
       uint64_t v = plan_bytes(shape, k);
       if (lanes) {
         uint64_t lp[3];
         lane_plan(shape, k, 2, 1, lp);
-        v += (uint64_t)lanes * lp[1];
+        v += (uint64_t)lanes * lp[1] + lane_sets;
       }
       return v;
     };
@@ -797,7 +803,9 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
       else if (fits(3)) s->recompute = true;
       else
         BJ_FAIL(ctx, BJ_ERR_OOM, plan_message("bj_setup_create", need, s->limit) +
-                                     (lanes ? " (each plan counted with the " + std::to_string(lanes) + " lane(s) of the context)" : std::string()));
+                                     (lanes ? " (each plan counted with the " + std::to_string(lanes) + " lane(s) of the context" +
+                                                  (lane_sets ? " and their witness slot sets of " + std::to_string(lane_sets) + " bytes)" : std::string(")"))
+                                            : std::string()));
     }
     if (ctx->comm && ctx->allow_sharded_recompute_plan && comm_world(ctx) > 1) {
       // The resident and streamed plans share their LDEs' monomials (lde_columns: every rank interpolates a block of the
@@ -1913,18 +1921,22 @@ int32_t bj_ctx_create_lane(bj_ctx* parent, bj_ctx** out) {
   {
     // every setup of the parent, with the lanes alive, this one, and the parent itself (its pool keeps what its setup and its
     // own proofs reached, so it counts as one proving context) must fit under the limit its plan was chosen under
+    // (and the witness slot sets alive on the lanes)
     std::lock_guard<std::mutex> lock(parent->tables_mu);
     const uint32_t lanes_after = parent->lanes.load() + 1;
+    const uint64_t lane_sets = parent->lane_witness_set_bytes;
     for (const bj_setup* s : parent->setups) {
       ProofShape sh;
       BJ_TRY(setup_shape(s, &sh));
       uint64_t p[3];
       lane_plan(sh, setup_plan_kind(s), s->chunk, lanes_after + 1, p);
       const uint64_t limit = parent->memory_limit ? parent->memory_limit : s->limit;
-      if (p[2] > limit)
+      if (p[2] + lane_sets > limit)
         BJ_FAIL(parent, BJ_ERR_OOM, "bj_ctx_create_lane: the setup's plan needs " + std::to_string(s->chosen_bytes()) + " bytes and every lane " +
                                         std::to_string(p[1]) + " bytes more; with " + std::to_string(lanes_after) + " lane(s) that is " +
-                                        std::to_string(p[2]) + " bytes, above the limit of " + std::to_string(limit) + " bytes");
+                                        std::to_string(p[2]) + " bytes" +
+                                        (lane_sets ? ", and the lanes' witness slot sets " + std::to_string(lane_sets) + " bytes" : std::string()) +
+                                        ", above the limit of " + std::to_string(limit) + " bytes");
     }
   }
   return ctx_new_lane(parent, out);

@@ -8,6 +8,8 @@
 // and is gathered into the slot on the copy stream through the setup's u32 copy hint (materialize_variables_polynomials_from_
 // dense_hint, witness.rs:325-385); the next upload overwrites all_values only after that gather, by the copy stream's order.
 // Pageable host memory is copied through a ring of pinned staging chunks on the calling thread (no helper thread).
+// A slot set may also live on a lane of the setup's context (bj_ctx_create_lane): its buffers come from the lane's pool, its
+// uploads run on the lane's own copy stream and its proofs on the lane's stream, so each lane streams its own witnesses.
 
 namespace bj {
 
@@ -38,17 +40,28 @@ __global__ void __launch_bounds__(256) widen_multiplicities_kernel(const u32* __
   out[i] = i < n_mult ? (u64)m[i] : 0;
 }
 
-// pool bytes of a slot set: the slots; with max_values > 0 the all_values buffer, the u32 multiplicities (lookup) and the u32
-// hint at its largest (n rows), each counted as one pool allocation the way pool_peak counts them
-static u64 witness_slots_pool_bytes(const bj_circuit& c, uint32_t n_slots, uint64_t max_values) {
+// pool bytes the set itself allocates in its context's pool: the slots; with max_values > 0 the all_values buffer and the u32
+// multiplicities (lookup); each counted as one pool allocation the way pool_peak counts them
+static u64 witness_slots_own_bytes(const bj_circuit& c, uint32_t n_slots, uint64_t max_values) {
   const u64 n = 1ull << c.log_n, lk = c.lookup_width ? 1 : 0;
   u64 b = pool_bytes((u64)n_slots * (c.num_variables + lk) * n);
   if (max_values) {
     b += pool_bytes(max_values);
-    b += pool_bytes(((u64)c.num_variables * n + 1) / 2);
     if (lk) b += pool_bytes((n + 1) / 2);
   }
   return b;
+}
+
+// the u32 hint at its largest (n rows), which bj_setup_attach_variables_hint allocates once, on the setup
+static u64 witness_hint_bytes(const bj_circuit& c) { return pool_bytes(((u64)c.num_variables * (1ull << c.log_n) + 1) / 2); }
+
+// pool bytes of a slot set on a parent: its own buffers, and with max_values > 0 the hint
+static u64 witness_slots_pool_bytes(const bj_circuit& c, uint32_t n_slots, uint64_t max_values) {
+  return witness_slots_own_bytes(c, n_slots, max_values) + (max_values ? witness_hint_bytes(c) : 0);
+}
+
+static bool witness_shape_valid(const bj_circuit* c, uint32_t n_slots) {
+  return c && n_slots && n_slots <= WITNESS_MAX_SLOTS && c->num_variables && c->log_n && c->log_n <= 28;
 }
 
 }  // namespace bj
@@ -59,6 +72,7 @@ struct bj_witness_slots {
   uint32_t n_slots = 0;
   uint64_t max_values = 0;
   uint64_t slot_len = 0;  // u64 of one slot: (V + lookup) * n
+  uint64_t counted = 0;   // pool bytes the set counts on its context (bj_ctx::witness_set_bytes)
   bj::DevMem slots, values, mult32;
   cudaEvent_t ready[bj::WITNESS_MAX_SLOTS] = {}, freed[bj::WITNESS_MAX_SLOTS] = {};
   bool filled[bj::WITNESS_MAX_SLOTS] = {};
@@ -158,6 +172,13 @@ int32_t bj_setup_attach_variables_hint(bj_setup* setup, const uint64_t* h_hint, 
   uint64_t need = 0;
   if (bj_variables_hint_to_u32(h_hint, cells, h32.data(), &need) != BJ_OK)
     BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_setup_attach_variables_hint: a variable index does not fit the u32 hint (>= 2^32 - 1)");
+  {
+    // a gather on a lane's copy stream may read the current hint; only the parent's streams are drained below
+    std::lock_guard<std::mutex> lock(ctx->tables_mu);
+    if (ctx->lane_witness_sets)
+      BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_setup_attach_variables_hint: " + std::to_string(ctx->lane_witness_sets) +
+                                           " witness slot set(s) of the context's lanes are alive: attach the hint before creating them");
+  }
   BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // a previous hint may still be read by a gather
   if (ctx->witness_stream) BJ_CUDA(ctx, cudaStreamSynchronize(ctx->witness_stream));
   BJ_TRY(setup->vars_hint.alloc(ctx, (cells + 1) / 2));
@@ -170,33 +191,91 @@ int32_t bj_setup_attach_variables_hint(bj_setup* setup, const uint64_t* h_hint, 
 }
 
 int32_t bj_witness_slots_bytes(const bj_circuit* c, uint32_t world, uint32_t n_slots, uint64_t max_values, uint64_t* out) {
-  if (!c || !out || world == 0 || (world & (world - 1)) || n_slots == 0 || n_slots > WITNESS_MAX_SLOTS || c->num_variables == 0 ||
-      c->log_n == 0 || c->log_n > 28)
-    return BJ_ERR_INVALID_ARG;
+  if (!out || world == 0 || (world & (world - 1)) || !witness_shape_valid(c, n_slots)) return BJ_ERR_INVALID_ARG;
   *out = witness_slots_pool_bytes(*c, n_slots, max_values);  // every rank holds the whole witness: the same on each of `world` GPUs
   return BJ_OK;
+}
+
+int32_t bj_witness_slots_bytes_split(const bj_circuit* c, uint32_t n_slots, uint64_t max_values, uint64_t out[2]) {
+  if (!out || !witness_shape_valid(c, n_slots)) return BJ_ERR_INVALID_ARG;
+  out[0] = witness_slots_own_bytes(*c, n_slots, max_values);
+  out[1] = max_values ? witness_hint_bytes(*c) : 0;
+  return BJ_OK;
+}
+
+// the memory check of a slot set on a lane, and its bytes counted on the lane and the parent (under the parent's tables_mu, so
+// that sets created at once on several lanes are checked against one another).  Everything that shares the limit is summed:
+// the setup with the live lanes and the parent proving at once, the hint once, the parent's sets, the lanes' sets, this set.
+static int32_t lane_witness_slots_reserve(bj_ctx* lane, const bj_setup* setup, uint32_t n_slots, uint64_t max_values, uint64_t* counted) {
+  bj_ctx* parent = lane->parent;
+  const bj_circuit& c = setup->c;
+  const uint64_t own = witness_slots_own_bytes(c, n_slots, max_values);
+  ProofShape sh;
+  BJ_TRY(setup_shape(setup, &sh));
+  std::lock_guard<std::mutex> lock(parent->tables_mu);
+  const uint32_t m = parent->lanes.load();
+  uint64_t p[3];
+  lane_plan(sh, setup_plan_kind(setup), setup->chunk, m + 1, p);
+  const uint64_t hint = max_values || setup->has_hint ? witness_hint_bytes(c) : 0;
+  const uint64_t total = p[2] + hint + parent->witness_set_bytes + parent->lane_witness_set_bytes + own;
+  const uint64_t limit = parent->memory_limit ? parent->memory_limit : setup->limit;
+  if (total > limit)
+    BJ_FAIL(lane, BJ_ERR_OOM, "bj_witness_slots_create: on a lane, the setup with " + std::to_string(m) + " lane(s) and the parent proving needs " +
+                                  std::to_string(p[2]) + " bytes, the variables hint " + std::to_string(hint) + " bytes, the parent's slot sets " +
+                                  std::to_string(parent->witness_set_bytes) + " bytes, the lanes' slot sets " +
+                                  std::to_string(parent->lane_witness_set_bytes) + " bytes and " + std::to_string(n_slots) + " witness slots " +
+                                  std::to_string(own) + " bytes: " + std::to_string(total) + " bytes, above the limit of " + std::to_string(limit) +
+                                  " bytes");
+  lane->witness_sets++;
+  lane->witness_set_bytes += own;
+  parent->lane_witness_sets++;
+  parent->lane_witness_set_bytes += own;
+  *counted = own;
+  return BJ_OK;
+}
+
+// takes back what a set counted on its context (and, for a lane, on the parent)
+static void witness_slots_unreserve(bj_ctx* ctx, uint64_t counted) {
+  bj_ctx* owner = ctx->parent ? ctx->parent : ctx;
+  std::lock_guard<std::mutex> lock(owner->tables_mu);
+  ctx->witness_sets--;
+  ctx->witness_set_bytes -= counted;
+  if (ctx->parent) {
+    ctx->parent->lane_witness_sets--;
+    ctx->parent->lane_witness_set_bytes -= counted;
+  }
 }
 
 int32_t bj_witness_slots_create(bj_ctx* ctx, const bj_setup* setup, uint32_t n_slots, uint64_t max_values, bj_witness_slots** out) {
   bj::DeviceGuard device_guard(ctx);
   if (!ctx || !setup || !out) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_witness_slots_create: bad argument");
   *out = nullptr;
-  if (setup->ctx != ctx) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_witness_slots_create: the setup belongs to another context");
+  const bool lane = ctx->parent != nullptr;
+  if (setup->ctx != (lane ? ctx->parent : ctx)) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_witness_slots_create: the setup belongs to another context");
   if (n_slots == 0 || n_slots > WITNESS_MAX_SLOTS) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_witness_slots_create: 1 to 4 slots");
   const bj_circuit& c = setup->c;
-  const uint64_t bytes = witness_slots_pool_bytes(c, n_slots, max_values);
-  {
+  uint64_t counted = 0;
+  if (lane) {
+    BJ_TRY(lane_witness_slots_reserve(ctx, setup, n_slots, max_values, &counted));
+  } else {
+    const uint64_t bytes = witness_slots_pool_bytes(c, n_slots, max_values);
     const uint64_t limit = ctx->memory_limit ? ctx->memory_limit : setup->limit;
     if (setup->chosen_bytes() + bytes > limit)
       BJ_FAIL(ctx, BJ_ERR_OOM, "bj_witness_slots_create: the setup's plan needs " + std::to_string(setup->chosen_bytes()) + " bytes and " +
                                    std::to_string(n_slots) + " witness slots " + std::to_string(bytes) + " bytes, above the limit of " +
                                    std::to_string(limit) + " bytes");
+    std::lock_guard<std::mutex> lock(ctx->tables_mu);
+    ctx->witness_sets++;
+    ctx->witness_set_bytes += bytes;
+    counted = bytes;
   }
-  if (!ctx->witness_stream) BJ_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->witness_stream, cudaStreamNonBlocking));
-  std::unique_ptr<bj_witness_slots> s(new bj_witness_slots());
+  // from here on the set is counted: a failure below frees it with bj_witness_slots_free, which takes the count back
+  std::unique_ptr<bj_witness_slots, void (*)(bj_witness_slots*)> s(new bj_witness_slots(), bj_witness_slots_free);
   s->ctx = ctx;
+  s->counted = counted;
   s->setup = setup;
   s->n_slots = n_slots;
+  if (!ctx->witness_stream) BJ_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->witness_stream, cudaStreamNonBlocking));
   s->max_values = max_values;
   const u64 n = 1ull << c.log_n;
   s->slot_len = (u64)(c.num_variables + (c.lookup_width ? 1 : 0)) * n;
@@ -218,7 +297,7 @@ void bj_witness_slots_free(bj_witness_slots* s) {
   if (!s) return;
   bj_ctx* ctx = s->ctx;
   bj::DeviceGuard device_guard(ctx);
-  cudaStreamSynchronize(ctx->witness_stream);
+  if (ctx->witness_stream) cudaStreamSynchronize(ctx->witness_stream);
   cudaStreamSynchronize(ctx->stream);
   for (uint32_t i = 0; i < s->n_slots; i++) {
     if (s->ready[i]) cudaEventDestroy(s->ready[i]);
@@ -229,6 +308,7 @@ void bj_witness_slots_free(bj_witness_slots* s) {
       if (s->staged[i]) cudaEventDestroy(s->staged[i]);
     cudaFreeHost(s->staging);
   }
+  witness_slots_unreserve(ctx, s->counted);
   delete s;  // the device buffers go back to the context's pool, ordered on its stream
 }
 

@@ -149,6 +149,7 @@ SIGNATURES = {
     "bj_proof_to_json": (_i32, [_vp, _vp, _sz, ctypes.POINTER(_sz)]),
     "bj_proof_stage_seconds": (_i32, [_vp, _vp]),
     "bj_witness_slots_bytes": (_i32, [_vp, _u32, _u32, _u64, _vp]),
+    "bj_witness_slots_bytes_split": (_i32, [_vp, _u32, _u64, _vp]),
     "bj_witness_slots_create": (_i32, [_vp, _vp, _u32, _u64, _pp]),
     "bj_witness_slots_free": (None, [_vp]),
     "bj_witness_upload": (_i32, [_vp, _u32, _vp, _vp]),

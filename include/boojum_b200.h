@@ -123,8 +123,11 @@ BJ_API int32_t bj_ctx_memory_high_water(bj_ctx* ctx, uint64_t* bytes, int32_t re
  * exceeds the parent's limit (bj_ctx_set_memory_limit, else the one the setup was planned under): `lanes` counts the lanes
  * alive after this one, and the parent counts as one more because its pool keeps what its setup and its own proofs reached.
  * A bj_setup_create on a parent with lanes alive counts them too: each plan must fit with one lane part per live lane.
+ * Witness slot sets (bj_witness_slots_create) may live on a lane too, one copy stream per lane; the lane's thread alone
+ * touches them.  bj_ctx_create_lane and bj_setup_create also count the bytes of the slot sets alive on the lanes.
  * Create the lanes of one parent from one thread.  Teardown: bj_ctx_destroy(parent) refuses with BJ_ERR_INVALID_ARG while a
- * lane is alive (destroy the lanes first); a setup may be freed once every bj_prove that reads it has returned. */
+ * lane is alive (destroy the lanes first), and bj_ctx_destroy(lane) while a slot set of the lane is alive (free it first); a
+ * setup may be freed once every bj_prove that reads it has returned. */
 BJ_API int32_t bj_ctx_create_lane(bj_ctx* parent, bj_ctx** out_lane);
 
 /* ---- multi-GPU: communicator of the sharded prover (one process - or one thread - per GPU) ----
@@ -639,9 +642,25 @@ BJ_API int32_t bj_proof_stage_seconds(const bj_proof* proof, double out[6]);
  * those bytes exceed the context's limit (bj_ctx_set_memory_limit, else the limit the setup was planned under).  Free the slot
  * set before its setup and context (both drain its copy stream).  Argument errors return BJ_ERR_INVALID_ARG with a message
  * before any launch: another context's setup, a slot out of range, a slot never uploaded, a witness vector without hint or
- * buffer, a lookup without multiplicities. */
+ * buffer, a lookup without multiplicities.
+ * On a lane (bj_ctx_create_lane): `ctx` may be a lane of the setup's context.  The set's buffers then come from the lane's pool
+ * and its uploads run on a copy stream the lane owns (created by the lane's first set, destroyed with the lane); it has its
+ * own staging ring, all_values and u32 multiplicities, and a WitnessVec gather reads the setup's hint from the lane's copy
+ * stream.  Uploads, bj_witness_slot_columns and bj_prove_slot(lane, setup, set, slot) behave as on the parent, and the proofs
+ * are the bytes bj_prove(parent, setup, ...) returns, on every single-GPU plan.  Only the lane's thread touches its sets.  The
+ * memory check on a lane sums bj_proof_memory_plan_lanes(setup, m + 1)[2] (m = the parent's live lanes), the hint once
+ * (out[1] of bj_witness_slots_bytes_split, when max_values > 0 or the setup has a hint), the full bytes of the parent's live
+ * sets, out[0] of the live sets of its lanes and out[0] of the new set, and refuses with BJ_ERR_OOM, naming every term and
+ * allocating nothing, above the parent's limit (else the one the setup was planned under).  bj_prove_slot refuses with
+ * BJ_ERR_INVALID_ARG a set of another context: another lane's, a lane's on the parent, the parent's on a lane.
+ * bj_setup_attach_variables_hint refuses with BJ_ERR_INVALID_ARG while a lane of the setup's context has a set alive (attach
+ * the hint before creating lane sets); bj_ctx_destroy(lane) refuses while a set of the lane is alive. */
 typedef struct bj_witness_slots bj_witness_slots;
 BJ_API int32_t bj_witness_slots_bytes(const bj_circuit* circuit, uint32_t world, uint32_t n_slots, uint64_t max_values, uint64_t* out);
+/* bj_witness_slots_bytes at world 1 split in two (host only): out[0] the bytes the set itself allocates in its context's pool,
+ * out[1] the u32 variables hint at its largest, which lives once on the setup (0 when max_values == 0).  out[0] + out[1] equals
+ * bj_witness_slots_bytes(circuit, 1, ...).  A set on a lane counts out[0] only. */
+BJ_API int32_t bj_witness_slots_bytes_split(const bj_circuit* circuit, uint32_t n_slots, uint64_t max_values, uint64_t out[2]);
 BJ_API int32_t bj_witness_slots_create(bj_ctx* ctx, const bj_setup* setup, uint32_t n_slots, uint64_t max_values, bj_witness_slots** out);
 BJ_API void bj_witness_slots_free(bj_witness_slots* slots);
 /* columns from host memory into a slot: h_variables [V][n], h_multiplicities n values (NULL without a lookup) */
