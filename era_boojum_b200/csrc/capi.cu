@@ -85,6 +85,7 @@ int32_t ctx_new_lane(bj_ctx* parent, bj_ctx** out) {
   lane->l2_persist_bytes = parent->l2_persist_bytes;
   lane->l2_window_max = parent->l2_window_max;
   lane->ntt_use_v2 = parent->ntt_use_v2;
+  lane->ntt_col_fastest = parent->ntt_col_fastest;
   lane->ntt_max_tile_log = parent->ntt_max_tile_log;
   lane->ntt_pass1_w = parent->ntt_pass1_w;
   lane->ntt_chunk_mb = parent->ntt_chunk_mb;
@@ -195,6 +196,7 @@ int32_t bj_ctx_create(int32_t device, void* stream, bj_ctx** out_ctx) {
   if (ctx->ntt_max_tile_log > 14) ctx->ntt_max_tile_log = 14;
   ctx->ntt_pass1_w = env_int("BJ_NTT_PASS1_W", -1);
   ctx->ntt_use_v2 = env_int("BJ_NTT_V2", 1);
+  ctx->ntt_col_fastest = env_int("BJ_NTT_COL_FASTEST", -1);
   ctx->ntt_full_pow = env_int("BJ_NTT_FULL_POW", 1);
   ctx->ntt_bulk = env_int("BJ_NTT_BULK", 0);
   ctx->ntt_l2_persist = env_int("BJ_NTT_L2_PERSIST", 1);

@@ -132,6 +132,7 @@ struct bj_ctx {
   bool ntt_attr_set = false;
   std::vector<void*> attr_done;  // kernels whose smem attributes are set on this device
   int ntt_use_v2 = 1;            // BJ_NTT_V2=0 forces the generic pass kernel
+  int ntt_col_fastest = -1;      // BJ_NTT_COL_FASTEST: tile passes run column-fastest, -1 by the rule of launch_pass, else bit 0 front, bit 1 last
   int ntt_max_tile_log = 13;  // tunables (env BJ_NTT_*)
   int ntt_pass1_w = -1;
   int ntt_chunk_mb = 0;

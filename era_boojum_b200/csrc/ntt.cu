@@ -471,7 +471,8 @@ static int32_t launch_pass(bj_ctx* ctx, const NttPass& p, u32 n_cols) {
   // experiment: bulk-copy (TMA) staged contiguous pass, BJ_NTT_BULK=1 (ntt_v2.cuh)
   const bool bulk_ok = ctx->ntt_bulk && aligned && p.kind == PASS_TILE && p.w == 0 && p.scale_mode == SCALE_NONE &&
                        p.log_n - p.r0 - p.t == 0 && ((p.src_col_stride | p.dst_col_stride) & 15) == 0;
-  if (ctx->ntt_use_v2 && aligned && v2_shape_ok && ((bulk_ok && v2_bulk_lookup(p.t, &v2)) || v2_lookup(p.t, p.w, p.kind, &v2))) {
+  const bool bulk = ctx->ntt_use_v2 && aligned && v2_shape_ok && bulk_ok && v2_bulk_lookup(p.t, &v2);
+  if (bulk || (ctx->ntt_use_v2 && aligned && v2_shape_ok && v2_lookup(p.t, p.w, p.kind, &v2))) {
     bool known = false;
     for (void* f : ctx->attr_done) known |= (f == (void*)v2.fn);
     if (!known) {
@@ -479,6 +480,27 @@ static int32_t launch_pass(bj_ctx* ctx, const NttPass& p, u32 n_cols) {
       BJ_CUDA(ctx, cudaFuncSetAttribute((const void*)v2.fn, cudaFuncAttributePreferredSharedMemoryCarveout,
                                         cudaSharedmemCarveoutMaxShared));
       ctx->attr_done.push_back((void*)v2.fn);
+    }
+    // Column-fastest order: block w is tile w / n_cols of column w % n_cols, so the same tile of every column runs back to
+    // back and the tile's slices of the twiddle and coset-power tables come from DRAM once per batch instead of once per
+    // column.  By default the contiguous last passes take it (twiddle slices, 1-2 % faster), and the front passes whose
+    // coset-power table is larger than the L2 set-aside that pins it (from 2^22 on the H100, 6-9 % faster).  A front pass
+    // whose table stays in L2 keeps the tile-fastest order: there neighbouring tiles of one column, which share DRAM pages,
+    // running together is worth more (5-14 % slower otherwise).  BJ_NTT_COL_FASTEST = bit 0 front, bit 1 last forces it.
+    const bool is_last = p.log_n - p.r0 - p.t == 0;
+    bool col_fastest;
+    if (ctx->ntt_col_fastest >= 0) {
+      col_fastest = (ctx->ntt_col_fastest >> (is_last ? 1 : 0)) & 1;
+    } else {
+      const bool big_table = p.scale_mode == SCALE_FULL && (sizeof(u64) << p.log_n) > ctx->l2_persist_bytes;
+      col_fastest = is_last || big_table;
+    }
+    if (p.kind == PASS_TILE && !bulk && col_fastest && tiles * n_cols <= 0x7fffffffull) {
+      NttPass ps = p;
+      ps.n_cols = n_cols;
+      v2.fn<<<(unsigned)(tiles * n_cols), v2.threads, v2.smem, ctx->stream>>>(ps);
+      BJ_LAUNCH_CHECK(ctx);
+      return BJ_OK;
     }
     return launch_column_slices(ctx, p, n_cols, [&](const NttPass& ps, u32 cols) {
       v2.fn<<<dim3((unsigned)tiles, cols, 1), v2.threads, v2.smem, ctx->stream>>>(ps);

@@ -139,9 +139,13 @@ __device__ __forceinline__ void ntt_pass_v2_body(const NttPass& p) {
   extern __shared__ u64 sm[];
   constexpr int WM = (1 << W) - 1;
   const int tid = threadIdx.x;
-  const u32 tile = blockIdx.x;
-  const u64* __restrict__ src = p.src + (u64)blockIdx.y * p.src_col_stride;
-  u64* __restrict__ dst = p.dst + (u64)blockIdx.y * p.dst_col_stride;
+  u32 tile = blockIdx.x, column = blockIdx.y;
+  if (KIND == PASS_TILE && p.n_cols) {
+    tile = blockIdx.x / p.n_cols;
+    column = blockIdx.x - tile * p.n_cols;
+  }
+  const u64* __restrict__ src = p.src + (u64)column * p.src_col_stride;
+  u64* __restrict__ dst = p.dst + (u64)column * p.dst_col_stride;
   const int m = p.log_n, r0 = p.r0;
   const bool scale_load = p.scale_mode != SCALE_NONE && p.scale_on_load;
   const bool scale_store = p.scale_mode != SCALE_NONE && !p.scale_on_load;
