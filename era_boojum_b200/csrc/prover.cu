@@ -15,7 +15,6 @@
 #include <functional>
 #include <memory>
 #include <string>
-#include <unordered_map>
 #include <vector>
 #include "ctx.hpp"
 
@@ -217,57 +216,6 @@ static int32_t lde_columns(bj_ctx* ctx, const uint64_t* d_in, uint64_t* d_out, u
   return finish(*groups.back());
 }
 
-// compact plan: the first `qn` elements (cosets [0, Q)) of every column, repacked with stride qn into `out`; cols is
-// repointed there.  The caller releases the full buffers.
-static int32_t keep_first_cosets(bj_ctx* ctx, std::vector<const uint64_t*>& cols, u64 qn, DevMem& out) {
-  BJ_TRY(out.alloc(ctx, cols.size() * qn));
-  for (size_t j = 0; j < cols.size(); j++) {
-    BJ_CUDA(ctx, cudaMemcpyAsync(out.p + j * qn, cols[j], sizeof(u64) * qn, cudaMemcpyDeviceToDevice, ctx->stream));
-    cols[j] = (const uint64_t*)out.p + j * qn;
-  }
-  return BJ_OK;
-}
-
-// compact plan: the witness and stage-2 LDEs are held as a few column groups, one allocation each, so that the repack to the
-// first Q cosets frees every group as soon as it is copied (the transient is one group's kept columns, not the oracle's)
-struct ColumnGroups {
-  std::vector<std::unique_ptr<DevMem>> full, kept;
-  std::vector<u32> cnt;
-};
-static constexpr u32 COMPACT_GROUPS = 4;
-static u32 compact_group_cols(u32 n_cols) { return (n_cols + COMPACT_GROUPS - 1) / COMPACT_GROUPS; }
-
-// LDE (one GPU) of n_cols natural columns of d_in onto all 2^log_d cosets, appended to g as groups; cols[j] = column j
-static int32_t lde_grouped(bj_ctx* ctx, ColumnGroups& g, const uint64_t* d_in, u32 n_cols, u32 log_n, u32 log_d, const uint64_t** cols) {
-  const u64 n = 1ull << log_n, nD = n << log_d;
-  const u32 per = compact_group_cols(n_cols);
-  for (u32 c0 = 0; c0 < n_cols; c0 += per) {
-    const u32 cnt = std::min(per, n_cols - c0);
-    g.full.emplace_back(new DevMem());
-    g.cnt.push_back(cnt);
-    BJ_TRY(g.full.back()->alloc(ctx, (size_t)cnt * nD));
-    BJ_TRY(bj_lde(ctx, d_in + (size_t)c0 * n, n, (uint64_t*)g.full.back()->p, log_n, log_d, cnt, 0));
-    for (u32 j = 0; j < cnt; j++) cols[c0 + j] = (const uint64_t*)g.full.back()->p + (size_t)j * nD;
-  }
-  return BJ_OK;
-}
-
-// keep_first_cosets group by group: cols (the groups' columns in order) is repointed to the kept copies
-static int32_t keep_first_cosets_grouped(bj_ctx* ctx, ColumnGroups& g, std::vector<const uint64_t*>& cols, u64 qn) {
-  size_t c0 = 0;
-  for (size_t k = 0; k < g.full.size(); k++) {
-    g.kept.emplace_back(new DevMem());
-    BJ_TRY(g.kept.back()->alloc(ctx, (size_t)g.cnt[k] * qn));
-    for (u32 j = 0; j < g.cnt[k]; j++) {
-      BJ_CUDA(ctx, cudaMemcpyAsync(g.kept.back()->p + (size_t)j * qn, cols[c0 + j], sizeof(u64) * qn, cudaMemcpyDeviceToDevice, ctx->stream));
-      cols[c0 + j] = (const uint64_t*)g.kept.back()->p + (size_t)j * qn;
-    }
-    g.full[k]->release();
-    c0 += g.cnt[k];
-  }
-  return BJ_OK;
-}
-
 int32_t copy_permutation_stage2_sharded(bj_ctx* ctx, const uint64_t* const* h_variable_cols, const uint64_t* const* h_sigma_cols, u32 n_cols,
                                         const uint64_t* h_non_residues, gl::e2 beta, gl::e2 gamma, u32 log_n, u32 chunk_size, u64* d_out);  // stage2.cu
 
@@ -400,6 +348,201 @@ struct Ledger {
     peak = std::max(peak, cur);
   }
   void sub(u64 n_u64) { cur -= pool_bytes(n_u64); }
+  void tree(const ProofShape& s) {  // oracle_build: leaf hashes, then the nodes
+    const u64 leaves = (s.n << s.log_l) / s.world;
+    add(4 * leaves);
+    add(4 * (leaves - s.cap / s.world));
+  }
+  void tree_by_coset(const ProofShape& s, u64 cols) {  // oracle_build_by_coset: leaf hashes, one unit of the columns, then the nodes
+    const u64 leaves = (s.n << s.log_l) / s.world, unit_rows = s.n >> (s.split + s.rb);
+    add(4 * leaves);
+    add(cols * unit_rows);
+    sub(cols * unit_rows);
+    add(4 * (leaves - s.cap / s.world));
+  }
+  void lde_groups(const ProofShape& s, u32 cols) {  // lde_columns on a sharded context: at most two column groups of monomials at once
+    const u64 w = s.world;
+    if (w == 1 || cols < 2) return;
+    const u64 group = std::max<u64>(w, ((cols + 3) / 4 + w - 1) / w * w), mono = w * ((group + w - 1) / w) * s.n;
+    const int alive = cols > group ? 2 : 1;
+    for (int i = 0; i < alive; i++) add(mono);
+    for (int i = 0; i < alive; i++) sub(mono);
+  }
+};
+
+// Every DevMem of bj_setup_create and bj_prove (and the FRI / query buffers of fri_driver.cu) is replayed by pool_peak in the
+// same order: the committed column sets' steps by ColumnSet::replay, beside them, the rest by pool_peak itself.  A new
+// allocation on either side must be added on the other, or the plan no longer bounds the pool (tests/test_gpu_memory_budget.py
+// pins the pool's high-water mark to the plan).
+
+// What one committed oracle (the setup, the witness or stage 2) keeps under the memory plan: its natural-order columns
+// (`nat`, stride n, in the oracle's column order), the LDE the plan keeps of them and the tree.  tree.cols are the kept LDE
+// columns (this context's units of the D cosets, of the L committed ones on the streamed plan, of cosets [0, Q) once the
+// compact plan has repacked them; stride `stride`) or, on the recompute plan, the natural-order columns themselves.  The LDE
+// is held in one allocation for all the spans (the setup) or one per span (the witness's variables and multiplicities, stage
+// 2), cut into column groups on the compact plan so that the repack to cosets [0, Q) frees each group as soon as it is copied
+// (the transient is one group's kept columns, not the oracle's).
+struct ColumnSet {
+  MemoryPlan plan = PLAN_RESIDENT;
+  std::vector<NatSpan> nat;
+  bool one_allocation = false;
+  u32 log_n = 0, log_l = 0, log_d = 0, Q = 0, rb = 0;
+  std::vector<std::unique_ptr<DevMem>> full, kept;  // the LDE's allocations, and on the compact plan their repacked copies
+  std::vector<u32> alloc_cols;                      // columns of each allocation
+  u64 stride = 0;
+  Oracle tree;
+
+  struct Piece {
+    u32 span, first, cnt;
+  };
+  static constexpr u32 COMPACT_GROUPS = 4;
+  // the LDE's allocations in order, each as the runs of span columns it holds
+  static std::vector<std::vector<Piece>> allocations(const std::vector<u32>& span_cols, bool one_allocation, MemoryPlan plan) {
+    std::vector<std::vector<Piece>> a;
+    for (u32 i = 0; i < span_cols.size(); i++) {
+      const u32 cnt = span_cols[i], per = plan == PLAN_COMPACT && !one_allocation ? (cnt + COMPACT_GROUPS - 1) / COMPACT_GROUPS : cnt;
+      for (u32 c0 = 0; c0 < cnt; c0 += per) {
+        if (a.empty() || !one_allocation) a.emplace_back();
+        a.back().push_back({i, c0, std::min(per, cnt - c0)});
+      }
+    }
+    return a;
+  }
+  static u64 cols_of(const std::vector<Piece>& a) {
+    u64 cols = 0;
+    for (const Piece& p : a) cols += p.cnt;
+    return cols;
+  }
+  // stride of an LDE column as first evaluated: D cosets, or on the streamed plan the L committed ones
+  static u64 evaluated_stride(MemoryPlan plan, u64 n, u32 log_l, u32 log_d, u32 world) { return (n << (plan == PLAN_STREAMED ? log_l : log_d)) / world; }
+
+  void init(MemoryPlan p, const ProofShape& s, std::vector<NatSpan> spans, bool one) {
+    plan = p;
+    nat = std::move(spans);
+    one_allocation = one;
+    log_n = s.log_n;
+    log_l = s.log_l;
+    log_d = s.log_d;
+    Q = s.Q;
+    rb = s.rb;
+  }
+  u32 size() const {
+    u32 cols = 0;
+    for (const NatSpan& sp : nat) cols += sp.cnt;
+    return cols;
+  }
+  const uint64_t* nat_col(u32 j) const {
+    for (const NatSpan& sp : nat) {
+      if (j < sp.cnt) return sp.p + ((size_t)j << log_n);
+      j -= sp.cnt;
+    }
+    return nullptr;
+  }
+  std::vector<u32> span_cols() const {
+    std::vector<u32> cols;
+    for (const NatSpan& sp : nat) cols.push_back(sp.cnt);
+    return cols;
+  }
+
+  // the LDE of the natural columns onto the cosets the plan evaluates (none on the recompute plan: its tree evaluates them
+  // a unit at a time)
+  int32_t evaluate(bj_ctx* ctx) {
+    if (plan == PLAN_RECOMPUTE) return BJ_OK;
+    const u32 log_kept = plan == PLAN_STREAMED ? log_l : log_d;
+    const u64 n = 1ull << log_n;
+    stride = evaluated_stride(plan, n, log_l, log_d, comm_world(ctx));
+    for (const auto& a : allocations(span_cols(), one_allocation, plan)) {
+      full.emplace_back(new DevMem());
+      alloc_cols.push_back((u32)cols_of(a));
+      BJ_TRY(full.back()->alloc(ctx, (size_t)alloc_cols.back() * stride));
+      uint64_t* out = (uint64_t*)full.back()->p;
+      for (const Piece& p : a) {
+        BJ_TRY(lde_columns(ctx, nat[p.span].p + (size_t)p.first * n, out, log_n, log_kept, p.cnt));
+        out += (size_t)p.cnt * stride;
+      }
+      for (u32 j = 0; j < alloc_cols.back(); j++) tree.cols.push_back((const uint64_t*)full.back()->p + (size_t)j * stride);
+    }
+    return BJ_OK;
+  }
+  int32_t build_tree(bj_ctx* ctx, u32 cap, u32 hasher) {
+    if (plan == PLAN_RECOMPUTE) return oracle_build_by_coset(ctx, tree, nat, log_n, log_l, cap, hasher, rb);
+    return oracle_build(ctx, tree, (1ull << log_n) << log_l, cap, hasher, 1u << log_l);
+  }
+  // compact plan: the first Q cosets of every column repacked with stride Q n, an allocation at a time; tree.cols repointed
+  int32_t keep_first_cosets(bj_ctx* ctx) {
+    if (plan != PLAN_COMPACT) return BJ_OK;
+    const u64 qn = (u64)Q << log_n;
+    size_t c0 = 0;
+    for (size_t k = 0; k < full.size(); k++) {
+      kept.emplace_back(new DevMem());
+      BJ_TRY(kept.back()->alloc(ctx, (size_t)alloc_cols[k] * qn));
+      for (u32 j = 0; j < alloc_cols[k]; j++) {
+        BJ_CUDA(ctx, cudaMemcpyAsync(kept.back()->p + (size_t)j * qn, tree.cols[c0 + j], sizeof(u64) * qn, cudaMemcpyDeviceToDevice, ctx->stream));
+        tree.cols[c0 + j] = (const uint64_t*)kept.back()->p + (size_t)j * qn;
+      }
+      full[k]->release();
+      c0 += alloc_cols[k];
+    }
+    stride = qn;
+    return BJ_OK;
+  }
+  // the kept stride matches a context of `world` ranks
+  bool built_for(u32 world) const {
+    const u64 n = 1ull << log_n;
+    return stride == (plan == PLAN_COMPACT ? (u64)Q * n : plan == PLAN_RECOMPUTE ? 0 : evaluated_stride(plan, n, log_l, log_d, world));
+  }
+  // the kept columns hold every local point of the quotient's cosets [0, Q)
+  bool keeps_quotient_cosets() const { return plan == PLAN_RESIDENT || plan == PLAN_COMPACT; }
+  // the natural columns are read again once the tree is built: the compact plan recomputes cosets [Q, L) from them, the
+  // streamed [L, Q), the recompute plan every coset
+  bool reads_natural() const { return plan != PLAN_RESIDENT; }
+  // the first of the `units` local committed units that DEEP and the queries rebuild from the natural columns (the compact
+  // plan keeps cosets [0, Q), the recompute plan none); `units` when every one is kept
+  u64 first_rebuilt(u64 units) const { return plan == PLAN_COMPACT ? Q : plan == PLAN_RECOMPUTE ? 0 : units; }
+  // the columns on local quotient unit k of `shard` (units of n >> shard.log_split rows; the caller sets the unit's window):
+  // on the streamed plan a unit of the committed cosets [0, L) is read from the kept columns, any other unit is evaluated
+  // from the natural columns into the next slots of `scratch` (bj_lde under the window: the same coset transform, or fold +
+  // row-block transform, as the resident plan's LDE)
+  int32_t quotient_unit(bj_ctx* ctx, const CosetShard& shard, u64 k, uint64_t*& scratch, std::vector<const uint64_t*>& out) const {
+    const u64 n = 1ull << log_n, ub = n >> shard.log_split;
+    out.clear();
+    if (plan == PLAN_STREAMED && k < shard.local_units(1ull << log_l)) {
+      for (const uint64_t* p : tree.cols) out.push_back(p + (size_t)k * ub);
+      return BJ_OK;
+    }
+    for (const NatSpan& sp : nat) {
+      if (sp.cnt) BJ_TRY(bj_lde(ctx, sp.p, n, scratch, log_n, log_d, sp.cnt, 0));
+      for (u32 i = 0; i < sp.cnt; i++) out.push_back(scratch + (size_t)i * ub);
+      scratch += (size_t)sp.cnt * ub;
+    }
+    return BJ_OK;
+  }
+
+  // pool_peak's replay of evaluate, build_tree and keep_first_cosets for a set of spans of span_cols columns; before_tree
+  // replays what the driver allocates or frees between evaluate and build_tree
+  static void replay(Ledger& m, const ProofShape& s, MemoryPlan plan, const std::vector<u32>& span_cols, bool one_allocation,
+                     const std::function<void()>& before_tree = nullptr) {
+    const auto allocs = allocations(span_cols, one_allocation, plan);
+    const u64 nE = plan == PLAN_RECOMPUTE ? 0 : evaluated_stride(plan, s.n, s.log_l, s.log_d, s.world);
+    if (plan != PLAN_RECOMPUTE)
+      for (const auto& a : allocs) {
+        m.add(cols_of(a) * nE);
+        for (const Piece& p : a) m.lde_groups(s, p.cnt);
+      }
+    if (before_tree) before_tree();
+    if (plan == PLAN_RECOMPUTE) {
+      u64 cols = 0;
+      for (u32 c : span_cols) cols += c;
+      m.tree_by_coset(s, cols);
+    } else {
+      m.tree(s);
+    }
+    if (plan == PLAN_COMPACT)
+      for (const auto& a : allocs) {
+        m.add(cols_of(a) * s.n * s.Q);
+        m.sub(cols_of(a) * nE);
+      }
+  }
 };
 
 // peak pool bytes of bj_setup_create followed by bj_prove; `chunk`: columns recomputed at a time (compact and recompute plans);
@@ -407,94 +550,32 @@ struct Ledger {
 static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk, u64* setup_held = nullptr) {
   Ledger m;
   const bool compact = plan == PLAN_COMPACT, streamed = plan == PLAN_STREAMED, recompute = plan == PLAN_RECOMPUTE;
-  const u64 n = s.n, w = s.world, nL = (n << s.log_l) / w, nQ = n << s.log_q, Qn = n * s.Q;
-  const u64 nD = streamed ? nL : (n << s.log_d) / w;  // elements of an LDE column as first evaluated
+  const u64 n = s.n, w = s.world, nL = (n << s.log_l) / w, nQ = n << s.log_q;
+  const u64 nD = (n << s.log_d) / w;
+  const u64 unit_rows = n >> (s.split + s.rb);  // rows of a quotient unit on the recompute plan
   const u64 leaves = (n << s.log_l) / w, capl = s.cap / w;
-  auto tree = [&]() {
-    m.add(4 * leaves);
-    m.add(4 * (leaves - capl));
-  };
-  const u64 unit_rows = n >> (s.split + s.rb);  // rows of a tree or quotient unit on the recompute plan
-  auto tree_by_coset = [&](u64 cols) {  // oracle_build_by_coset: leaf hashes, one unit of the columns, then the nodes
-    m.add(4 * leaves);
-    m.add(cols * unit_rows);
-    m.sub(cols * unit_rows);
-    m.add(4 * (leaves - capl));
-  };
   auto rebuild_chunks = [&]() {  // for_chunks: the monomials and one unit (a coset, or a row block) of a chunk of natural columns
     m.add((u64)chunk * n);
     m.add((u64)chunk * (n >> s.split));
     m.sub((u64)chunk * (n >> s.split));
     m.sub((u64)chunk * n);
   };
-  auto lde_groups = [&](u32 cols) {  // lde_columns on a sharded context: at most two column groups of monomials at once
-    if (w == 1 || cols < 2) return;
-    const u64 group = std::max<u64>(w, ((cols + 3) / 4 + w - 1) / w * w), mono = w * ((group + w - 1) / w) * n;
-    const int alive = cols > group ? 2 : 1;
-    for (int i = 0; i < alive; i++) m.add(mono);
-    for (int i = 0; i < alive; i++) m.sub(mono);
-  };
   const u64 S = s.V + s.C + s.T;
   // bj_setup_create
-  if (recompute) {
-    tree_by_coset(S);
-  } else {
-    m.add(S * nD);
-    lde_groups(s.V);
-    lde_groups(s.C);
-    lde_groups(s.T);
-    tree();
-  }
-  if (compact) {
-    m.add(S * Qn);
-    m.sub(S * nD);
-  }
+  ColumnSet::replay(m, s, plan, {s.V, s.C, s.T}, true);
   if (setup_held) *setup_held = m.cur;
-  // the compact plan's column groups (lde_grouped / keep_first_cosets_grouped): sizes of the groups of n_cols columns
-  auto groups = [](u32 n_cols) {
-    std::vector<u64> g;
-    for (u32 c0 = 0, per = compact_group_cols(n_cols); c0 < n_cols; c0 += per) g.push_back(std::min(per, n_cols - c0));
-    return g;
-  };
-  std::vector<u64> wg = groups(s.V), sg = groups(s.n_s2);
-  if (s.lk) wg.push_back(1);
   // round 1
-  if (recompute) {
-    tree_by_coset(s.W);
-  } else if (compact) {
-    for (u64 g : wg) m.add(g * nD);
-  } else {
-    m.add(s.V * nD);
-    lde_groups(s.V);
-    if (s.lk) m.add(nD);
-  }
-  if (!recompute) tree();
-  if (compact)
-    for (u64 g : wg) {
-      m.add(g * Qn);
-      m.sub(g * nD);
-    }
-  // round 2
+  ColumnSet::replay(m, s, plan, {s.V, s.lk ? 1u : 0u}, false);
+  // round 2: the natural stage-2 columns, then their set, with z(omega x) on a split shard of the resident plan (the streamed
+  // and recompute plans evaluate it per unit, into their scratch) between evaluation and tree
   m.add(s.n_s2 * n);
-  if (recompute) {
-    tree_by_coset(s.n_s2);
-  } else if (compact) {
-    for (u64 g : sg) m.add(g * nD);
-  } else {
-    m.add(s.n_s2 * nD);
-    lde_groups(s.n_s2);
-  }
-  const u64 zn = s.split && !streamed && !recompute ? 2 * nD : 0;  // the streamed and recompute plans evaluate z(omega x) per unit, into their scratch
-  if (zn) m.add(zn);
-  // the compact plan keeps the natural stage-2 columns for DEEP and the queries, the streamed plan for the quotient, the
-  // recompute plan for both
-  if (!compact && !streamed && !recompute) m.sub(s.n_s2 * n);
-  if (!recompute) tree();
-  if (compact)
-    for (u64 g : sg) {
-      m.add(g * Qn);
-      m.sub(g * nD);
-    }
+  const u64 zn = s.split && !streamed && !recompute ? 2 * nD : 0;
+  ColumnSet::replay(m, s, plan, {s.n_s2}, false, [&]() {
+    if (zn) m.add(zn);
+    // the compact plan keeps the natural stage-2 columns for DEEP and the queries, the streamed plan for the quotient, the
+    // recompute plan for both
+    if (!compact && !streamed && !recompute) m.sub(s.n_s2 * n);
+  });
   // round 3
   m.add(2 * nQ);
   const u64 nQl = ((u64)s.Q << s.split) >= w ? nQ / w : n >> s.split;
@@ -517,7 +598,7 @@ static u64 pool_peak(const ProofShape& s, MemoryPlan plan, u32 chunk, u64* setup
   m.sub(2 * nQ);  // qq
   m.add(2 * (u64)s.Q * nL);
   m.sub(2 * nQ);  // chunks
-  tree();
+  m.tree(s);
   // round 4: the recompute plan opens the natural columns on coset 0, rebuilt a chunk at a time
   if (recompute) rebuild_chunks();
   // round 5
@@ -610,15 +691,17 @@ struct bj_setup {
   std::vector<uint32_t> pi_cols, pi_rows;
   const uint64_t *sigmas = nullptr, *constants = nullptr, *tables = nullptr;  // borrowed, natural row order
   uint32_t n_tables = 0;
-  bj::DevMem lde;  // [V + C + T][D][n], D = max(L, quotient degree): the tree commits to the first L cosets of every column
-  bj::Oracle tree;
-  uint64_t col_len = 0;  // elements of one LDE column held by this context: n * (D / world), n * Q compact, n * (L / world) streamed, 0 recompute
-  bool compact = false;   // memory plan chosen by bj_setup_create, followed by bj_prove
-  bool streamed = false;
-  bool recompute = false;
+  // [V + C + T] sigmas | constants | tables and the setup tree.  The reference evaluates at D = max(fri_lde_factor, quotient
+  // degree) and commits to the subset of the first fri_lde_factor cosets (prover.rs:178-196 `used_lde_degree`,
+  // `subset_for_degree`): in the bit-reversed coset order the first L cosets of the factor-D domain ARE the factor-L domain,
+  // so the trees, DEEP, FRI and the queries work on the prefix [0, n * L) of every column and only the quotient stage reads
+  // the cosets beyond it.
+  bj::ColumnSet cols;
+  bj::MemoryPlan plan = bj::PLAN_RESIDENT;  // chosen by bj_setup_create, followed by bj_prove
+  bj::ProofShape shape{};                   // the proof's shape on this context, with the chosen row blocks
   uint32_t log_blocks = 0;  // recompute plan on one GPU: log2 of the row blocks per coset (bj_setup_row_blocks), 0 elsewhere
   uint64_t limit = 0;    // the device-memory limit the plan was chosen under
-  uint64_t plan[4] = {0, 0, 0, 0};  // resident, compact, streamed, recompute (0: the plan does not apply or was not allowed)
+  uint64_t plan_bytes[4] = {0, 0, 0, 0};  // resident, compact, streamed, recompute (0: the plan does not apply or was not allowed)
   uint32_t chunk = 2;         // compact and recompute plans: natural-order columns recomputed at a time
   uint64_t pool_bytes = 0, outside_pool_bytes = 0;  // the chosen plan (with its chunk): pool peak, library reserve
   uint64_t chosen_bytes() const { return pool_bytes + outside_pool_bytes; }
@@ -628,21 +711,6 @@ struct bj_setup {
   uint64_t hint_values = 0;  // 1 + the largest index the hint names: an all_values vector needs at least this many values
   bool has_hint = false;
   cudaEvent_t ready = nullptr;  // recorded on the context's stream when bj_setup_create returns: bj_prove on a lane waits for it
-  const uint64_t* col(uint32_t j) const { return (const uint64_t*)lde.p + (size_t)j * col_len; }
-  uint32_t log_l() const {
-    uint32_t l = 0;
-    while ((1u << l) < c.fri_lde_factor) l++;
-    return l;
-  }
-  // log2 of the LDE factor the columns are evaluated at.  The reference evaluates at max(fri_lde_factor, quotient degree) and
-  // commits to the subset of the first fri_lde_factor cosets (prover.rs:178-196 `used_lde_degree`, `subset_for_degree`): in the
-  // bit-reversed coset order the first L cosets of the factor-D domain ARE the factor-L domain, so the trees, DEEP, FRI and
-  // the queries work on the prefix [0, n * L) of every column and only the quotient stage reads the cosets beyond it.
-  uint32_t log_d() const {
-    uint32_t l = log_l();
-    while ((1u << l) < c.quotient_degree) l++;
-    return l;
-  }
 };
 
 struct bj_proof {
@@ -691,6 +759,881 @@ static std::string plan_message(const char* who, const uint64_t plan[4], uint64_
   if (plan[2]) m += " and " + std::to_string(plan[2]) + " bytes on the streamed plan";
   if (plan[3]) m += " and " + std::to_string(plan[3]) + " bytes on the recompute plan";
   return m + ", above the limit of " + std::to_string(limit) + " bytes";
+}
+
+
+// The memory plan: resident if it fits under the limit, else compact (Q < L, one GPU), else streamed (Q > L), else recompute
+// (one GPU when the context allows it, a context with a communicator when it allows the sharded recompute plan); refused
+// before anything is launched.  On a sharded context every rank chooses under its own limit: every plan commits to the same
+// units and runs the same collectives, so ranks on different plans still agree.  Sets s->plan, plan_bytes, limit, log_blocks,
+// chunk, the chosen bytes and s->shape, the proof's shape with the chosen row blocks.
+static int32_t choose_plan(bj_ctx* ctx, const bj_circuit* circuit, bj_setup* s) {
+  ProofShape sh;
+  BJ_TRY(proof_shape(*circuit, comm_world(ctx), &sh));
+  s->plan_bytes[0] = plan_bytes(sh, PLAN_RESIDENT);
+  s->plan_bytes[1] = compact_applies(sh) ? plan_bytes(sh, PLAN_COMPACT) : 0;
+  s->plan_bytes[2] = streamed_applies(sh) ? plan_bytes(sh, PLAN_STREAMED) : 0;
+  const bool recompute_allowed = (ctx->allow_recompute_plan && recompute_applies(sh)) ||
+                                 (ctx->allow_sharded_recompute_plan && ctx->comm && recompute_sharded_applies(sh));
+  BJ_TRY(memory_limit(ctx, &s->limit));
+  // with lanes alive on the context, a plan must also hold their proofs: one lane part each beside the plan, and the
+  // witness slot sets alive on the lanes
+  const uint32_t lanes = ctx->lanes.load();
+  uint64_t lane_sets = 0;
+  {
+    std::lock_guard<std::mutex> lock(ctx->tables_mu);
+    lane_sets = ctx->lane_witness_set_bytes;
+  }
+  auto need_of = [&](const ProofShape& shape, MemoryPlan k) {
+    uint64_t v = plan_bytes(shape, k);
+    if (lanes) {
+      uint64_t lp[3];
+      lane_plan(shape, k, 2, 1, lp);
+      v += (uint64_t)lanes * lp[1] + lane_sets;
+    }
+    return v;
+  };
+  uint64_t need[4];
+  for (int k = 0; k < 3; k++) need[k] = s->plan_bytes[k] ? need_of(sh, (MemoryPlan)k) : 0;
+  // the recompute plan on one GPU: the fewest row blocks per coset (up to the context's bj_ctx_set_max_row_blocks) whose
+  // plan fits, or the most allowed when none does, so that a refusal names the smallest recompute plan on offer
+  uint32_t rb = 0;
+  need[3] = 0;
+  if (recompute_allowed) {
+    uint32_t max_rb = 0;
+    while (!ctx->comm && (2u << max_rb) <= ctx->max_row_blocks && row_blocks_valid(sh, max_rb + 1)) max_rb++;
+    ProofShape shb = sh;
+    for (;; rb++) {
+      shb.rb = rb;
+      need[3] = need_of(shb, PLAN_RECOMPUTE);
+      if (need[3] <= s->limit || rb == max_rb) break;
+    }
+    s->plan_bytes[3] = plan_bytes(shb, PLAN_RECOMPUTE);
+  }
+  auto fits = [&](int k) { return need[k] && need[k] <= s->limit; };
+  if (need[0] > s->limit) {
+    if (fits(2)) s->plan = PLAN_STREAMED;
+    else if (fits(1)) s->plan = PLAN_COMPACT;
+    else if (fits(3)) s->plan = PLAN_RECOMPUTE;
+    else
+      BJ_FAIL(ctx, BJ_ERR_OOM, plan_message("bj_setup_create", need, s->limit) +
+                                   (lanes ? " (each plan counted with the " + std::to_string(lanes) + " lane(s) of the context" +
+                                                (lane_sets ? " and their witness slot sets of " + std::to_string(lane_sets) + " bytes)" : std::string(")"))
+                                          : std::string()));
+  }
+  if (ctx->comm && ctx->allow_sharded_recompute_plan && comm_world(ctx) > 1) {
+    // The resident and streamed plans share their LDEs' monomials (lde_columns: every rank interpolates a block of the
+    // columns, one all-gather per column group); the recompute plan evaluates its units from the natural-order columns and
+    // takes part in no such exchange.  So the ranks agree before their first collective: once one rank needs the recompute
+    // plan every rank takes it (a proof runs at its slowest rank's pace, so this costs the others no time), or, where a
+    // rank's limit does not hold it, every rank refuses.
+    const uint32_t world = comm_world(ctx);
+    const u64 mine[2] = {s->plan == PLAN_RECOMPUTE ? 1u : 0u, fits(3) ? 1u : 0u};
+    std::vector<u64> all(2 * (size_t)world);
+    BJ_TRY(comm_all_gather_host(ctx->comm, mine, all.data(), 2));
+    bool any = false, every = true;
+    for (uint32_t r = 0; r < world; r++) {
+      any = any || all[2 * r];
+      every = every && all[2 * r + 1];
+    }
+    if (any && !every)
+      BJ_FAIL(ctx, BJ_ERR_OOM, "bj_setup_create: a rank needs the recompute plan and another rank's limit does not hold it; " +
+                                   plan_message("this rank", need, s->limit));
+    if (any) s->plan = PLAN_RECOMPUTE;
+  }
+  if (s->plan == PLAN_RECOMPUTE) s->log_blocks = rb;
+  sh.rb = s->log_blocks;
+  if (s->plan == PLAN_COMPACT || s->plan == PLAN_RECOMPUTE) {
+    // wider recompute chunks only save kernel launches: the chunk grows into at most half of the headroom the limit leaves
+    // over the plan (the rest is slack for the pool's fragmentation) and stops at 16 columns
+    const uint64_t planned = s->plan_bytes[s->plan];
+    const uint64_t budget = planned + (s->limit - planned) / 2;
+    uint32_t lo = 2, hi = std::max<uint32_t>(2, std::min<uint32_t>(16, sh.nat_cols()));
+    while (lo < hi) {
+      const uint32_t mid = lo + (hi - lo + 1) / 2;
+      if (plan_bytes(sh, s->plan, mid) <= budget) lo = mid;
+      else hi = mid - 1;
+    }
+    s->chunk = lo;
+  }
+  s->pool_bytes = pool_peak(sh, s->plan, s->chunk);
+  s->outside_pool_bytes = library_reserve(sh);
+  s->shape = sh;
+  return BJ_OK;
+}
+
+// the proof's oracles, in the order of a query's answer
+enum OracleId : u32 { WITNESS, STAGE2, QUOTIENT, SETUP };
+
+// a polynomial opened and added to DEEP: column `col` of an oracle, or an Fp2 one (ext): columns col (c0) and col + 1 (c1)
+struct Src {
+  u32 oracle, col;
+  bool ext;
+};
+
+// One proof (bj_prove): the transcript, the proof, the column sets and the quotient oracle, the challenges, round by round
+struct Prover {
+  bj_ctx* ctx;
+  const bj_setup& setup;
+  const bj_circuit& c;
+  const uint64_t *d_variables, *d_multiplicities;
+  bj_proof& pf;
+  bj_transcript* tr;
+  bj_fri_oracles* fri = nullptr;
+  uint32_t V, C, T, Q, L, cap, log_n, log_l, log_d, log_q, world, rank, split, wdt, nsub, voff, n_partial, n_s2, a_off;
+  bool lk;
+  u64 n, nQ, nL, nD, nQl, nb;
+  // domain shard (multi-GPU): this context holds (L << split) / world units of every LDE column and its units of the first
+  // Q cosets; nL, nD = its length of the committed part of an LDE column and of a whole one (D = max(L, Q)), nQl its quotient
+  // points, nb = n >> split the rows of a unit
+  ColumnSet witness, stage2;  // variables | multiplicities, and z | partials | A_i | B (c0, c1 each)
+  DevMem st2;                 // the natural-order stage-2 columns
+  DevMem z_next;              // split shard, resident plan: z(omega x) on this rank's cosets
+  DevMem qt_lde;
+  Oracle qt;
+  // DEEP and the queries rebuild the local committed units [first_rebuilt, units_l) of the setup, witness and stage-2
+  // columns from their natural-order columns, a chunk of the flat order setup | witness | stage 2 (oracle o's columns from
+  // base[o]) at a time
+  u64 units_l, first_rebuilt;
+  bool rebuild;
+  uint32_t base[4] = {0, 0, 0, 0}, n_rebuilt = 0;
+  gl::e2 beta, gamma, lookup_beta{0, 0}, lookup_gamma{0, 0}, z, z_omega;
+  std::vector<Src> sources, z_omega_sources, zero_sources;
+  DevMem deep;
+  uint32_t num_queries = 0, sched[32], sched_len = 0;
+
+  Prover(bj_ctx* x, const bj_setup& s, const uint64_t* vars, const uint64_t* mults, bj_proof& p)
+      : ctx(x), setup(s), c(s.c), d_variables(vars), d_multiplicities(mults), pf(p) {
+    tr = c.transcript == 1 ? bj_transcript_new_blake2s() : c.transcript == 2 ? bj_transcript_new_keccak256() : c.transcript == 3 ? bj_transcript_new_poseidon() : bj_transcript_new();
+    V = c.num_variables, C = c.num_constants, T = setup.n_tables, Q = c.quotient_degree, L = c.fri_lde_factor, cap = c.merkle_tree_cap_size;
+    log_n = c.log_n, log_l = setup.shape.log_l, log_d = setup.shape.log_d, log_q = setup.shape.log_q;
+    n = 1ull << log_n, nQ = n << log_q;
+    world = comm_world(ctx), rank = comm_rank(ctx);
+    nL = (n << log_l) / world, nD = (n << log_d) / world, nQl = ctx->shard.local_points(Q, (int)log_n);
+    split = ctx->shard.log_split, nb = n >> split;
+    lk = c.lookup_width != 0, wdt = c.lookup_width, nsub = c.lookup_num_repetitions, voff = c.lookup_variables_offset;
+    n_partial = (V + Q - 1) / Q - 1;
+    n_s2 = 2 + 2 * n_partial + (lk ? 2 * (nsub + 1) : 0);
+    a_off = 2 + 2 * n_partial;
+    units_l = ctx->shard.local_units(L);
+    first_rebuilt = setup.cols.first_rebuilt(units_l);
+    rebuild = first_rebuilt < units_l;
+    witness.init(setup.plan, setup.shape, {{d_variables, V}, {d_multiplicities, lk ? 1u : 0u}}, false);
+    base[WITNESS] = setup.cols.size();
+    base[STAGE2] = base[WITNESS] + witness.size();
+    n_rebuilt = base[STAGE2] + n_s2;
+  }
+  ~Prover() {
+    bj_fri_oracles_free(fri);
+    bj_transcript_free(tr);
+  }
+  Prover(const Prover&) = delete;
+  Prover& operator=(const Prover&) = delete;
+
+  gl::e2 challenge2() {
+    gl::e2 r;
+    r.c0 = bj_transcript_get_challenge(tr);
+    r.c1 = bj_transcript_get_challenge(tr);
+    return r;
+  }
+  const ColumnSet& set(uint32_t o) const { return o == SETUP ? setup.cols : o == WITNESS ? witness : stage2; }
+  const Oracle& oracle(uint32_t o) const { return o == QUOTIENT ? qt : set(o).tree; }
+  const uint64_t* col(uint32_t o, uint32_t j) const { return oracle(o).cols[j]; }
+  // every rebuilt column among [lo, hi) of the flat order: f(oracle, its column, flat index), in flat order
+  template <class F>
+  void for_flat(uint32_t lo, uint32_t hi, F&& f) const {
+    for (uint32_t o : {SETUP, WITNESS, STAGE2})
+      for (uint32_t i = std::max(lo, base[o]); i < std::min(hi, base[o] + set(o).size()); i++) f(o, i - base[o], i);
+  }
+  // flat column i and i + 1 are the c0, c1 of one Fp2 polynomial: stage 2 holds those pairs alone
+  bool pair_start(uint32_t i) const { return i >= base[STAGE2] && (i - base[STAGE2]) % 2 == 0; }
+
+  int32_t public_inputs() {
+    bj_transcript_witness_merkle_tree_cap(tr, (const uint64_t*)setup.cols.tree.cap.data(), cap);  // prover.rs:211
+    // public inputs: read from the witness, committed to before anything else (prover.rs:264-266)
+    const uint32_t n_pi = c.n_public_inputs;
+    pf.public_inputs.resize(n_pi);
+    for (uint32_t i = 0; i < n_pi; i++)
+      BJ_CUDA(ctx, cudaMemcpyAsync(&pf.public_inputs[i], d_variables + ((size_t)setup.pi_cols[i] << c.log_n) + setup.pi_rows[i], sizeof(u64),
+                                   cudaMemcpyDeviceToHost, ctx->stream));
+    if (n_pi) BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    for (uint32_t i = 0; i < n_pi; i++) {
+      pf.public_inputs[i] = gl::canon(pf.public_inputs[i]);
+      const uint64_t v = pf.public_inputs[i];
+      bj_transcript_witness_field_elements(tr, &v, 1);
+    }
+    return BJ_OK;
+  }
+
+  // ---- round 1: witness commitment (variables | witness (none) | multiplicities) ----
+  int32_t round1() {
+    BJ_TRY(witness.evaluate(ctx));
+    BJ_TRY(witness.build_tree(ctx, cap, c.tree_hasher));
+    pf.witness_cap = witness.tree.cap;
+    bj_transcript_witness_merkle_tree_cap(tr, (const uint64_t*)witness.tree.cap.data(), cap);
+    return witness.keep_first_cosets(ctx);
+  }
+
+  // ---- round 2: copy-permutation grand product, partial products, lookup polynomials ----
+  int32_t round2() {
+    beta = challenge2();
+    gamma = challenge2();
+    if (lk) {
+      lookup_beta = challenge2();  // prover.rs:402-406
+      lookup_gamma = challenge2();
+    }
+    BJ_TRY(st2.alloc(ctx, (size_t)n_s2 * n));
+    std::vector<const uint64_t*> vp(V), sp(V);
+    for (uint32_t j = 0; j < V; j++) {
+      vp[j] = d_variables + (size_t)j * n;
+      sp[j] = setup.sigmas + (size_t)j * n;
+    }
+    std::vector<uint64_t> nr(V);
+    BJ_TRY(bj_non_residues_for_copy_permutation(n, V, nr.data()));
+    const uint64_t b[2] = {beta.c0, beta.c1}, g[2] = {gamma.c0, gamma.c1};
+    if (world > 1 && n >= (u64)world * 16)  // rows split over the ranks, one all-gather (stage2.cu)
+      BJ_TRY(copy_permutation_stage2_sharded(ctx, vp.data(), sp.data(), V, nr.data(), beta, gamma, log_n, Q, st2.p));
+    else
+      BJ_TRY(bj_copy_permutation_stage2(ctx, vp.data(), sp.data(), V, nr.data(), b, g, log_n, Q, (uint64_t*)st2.p, (uint64_t*)st2.p + n,
+                                        (uint64_t*)st2.p + 2 * n));
+    if (lk) {
+      std::vector<const uint64_t*> lc(wdt * nsub), tc(T);
+      for (uint32_t i = 0; i < wdt * nsub; i++) lc[i] = d_variables + (size_t)(voff + i) * n;
+      for (uint32_t j = 0; j < T; j++) tc[j] = setup.tables + (size_t)j * n;
+      const uint64_t lb[2] = {lookup_beta.c0, lookup_beta.c1}, lg[2] = {lookup_gamma.c0, lookup_gamma.c1};
+      BJ_TRY(bj_lookup_polys_specialized(ctx, lc.data(), nsub, wdt, setup.constants + (size_t)c.lookup_table_id_column * n, tc.data(), T,
+                                         d_multiplicities, lb, lg, log_n, (uint64_t*)st2.p + (size_t)a_off * n));
+    }
+    stage2.init(setup.plan, setup.shape, {{(const uint64_t*)st2.p, n_s2}}, false);
+    BJ_TRY(stage2.evaluate(ctx));
+    // a row block of a split shard does not hold z(omega x) (another block of the coset does).  On a unit with shift sigma,
+    // z(omega x) is the LDE of z on the shift sigma * omega in the same row order: two more columns (c0, c1 of z).  The
+    // streamed and recompute plans evaluate them one unit at a time with the quotient's other columns.
+    if (split && stage2.keeps_quotient_cosets() && ctx->shard.local_units(Q)) {
+      BJ_TRY(z_next.alloc(ctx, 2 * nD));
+      BJ_TRY(bj_lde_next_row(ctx, (const uint64_t*)st2.p, n, (uint64_t*)z_next.p, log_n, log_d, 2, 0));
+    }
+    if (!stage2.reads_natural()) st2.release();
+    BJ_TRY(stage2.build_tree(ctx, cap, c.tree_hasher));
+    pf.stage2_cap = stage2.tree.cap;
+    bj_transcript_witness_merkle_tree_cap(tr, (const uint64_t*)stage2.tree.cap.data(), cap);
+    BJ_TRY(stage2.keep_first_cosets(ctx));
+    return BJ_OK;
+  }
+
+  // ---- round 3: quotient ----
+  // the columns the quotient reads, on the points it evaluates: the setup's (sigmas | constants | tables), the witness's
+  // (variables | multiplicities) and stage 2's, and on a row block z(omega x)
+  struct QuotientCols {
+    const uint64_t* const* setup;
+    const uint64_t* const* w;
+    const uint64_t* const* s2;
+    const uint64_t *z_next0, *z_next1;
+  };
+  int32_t quotient_terms(const QuotientCols& k, const std::vector<uint64_t>& powers, uint32_t n_lk_terms, uint32_t n_gate_terms, u64 n_points,
+                         uint64_t* o0, uint64_t* o1) {
+    const uint64_t* const* consts = k.setup + V;
+    const uint64_t* const* tables = k.setup + V + C;
+    if (lk) {
+      std::vector<const uint64_t*> ll(wdt * nsub), al(2 * nsub);
+      for (uint32_t i = 0; i < wdt * nsub; i++) ll[i] = k.w[voff + i];
+      for (uint32_t i = 0; i < 2 * nsub; i++) al[i] = k.s2[a_off + i];
+      const uint64_t lb[2] = {lookup_beta.c0, lookup_beta.c1}, lg[2] = {lookup_gamma.c0, lookup_gamma.c1};
+      BJ_TRY(bj_quotient_lookup_specialized(ctx, ll.data(), nsub, wdt, consts[c.lookup_table_id_column], tables, T, k.w[V], al.data(),
+                                            k.s2[a_off + 2 * nsub], k.s2[a_off + 2 * nsub + 1], lb, lg, powers.data(), n_points, o0, o1));
+    }
+    if (n_gate_terms)
+      BJ_TRY(bj_quotient_gates_general_purpose(ctx, setup.gates.data(), (uint32_t)setup.gates.size(), k.w, V, nullptr, 0, consts, C,
+                                               powers.data() + 2 * (size_t)n_lk_terms, n_gate_terms, n_points, o0, o1));
+    std::vector<uint64_t> nr(V);
+    BJ_TRY(bj_non_residues_for_copy_permutation(n, V, nr.data()));
+    const uint64_t b[2] = {beta.c0, beta.c1}, g[2] = {gamma.c0, gamma.c1};
+    const uint64_t* copy_powers = powers.data() + 2 * (size_t)(n_lk_terms + n_gate_terms);
+    if (ctx->shard.log_split)  // a row block (split shard, or a recompute unit under its window) does not hold z(omega x)
+      BJ_TRY(bj_quotient_copy_permutation_with_z_next(ctx, k.w, k.setup, V, nr.data(), k.s2[0], k.s2[1], k.z_next0, k.z_next1,
+                                                      n_partial ? k.s2 + 2 : nullptr, b, g, copy_powers, log_n, log_d, log_q, Q, o0, o1));
+    else
+      BJ_TRY(bj_quotient_copy_permutation(ctx, k.w, k.setup, V, nr.data(), k.s2[0], k.s2[1], n_partial ? k.s2 + 2 : nullptr, b, g, copy_powers,
+                                          log_n, log_d, log_q, Q, o0, o1));
+    return bj_quotient_divide_by_vanishing(ctx, o0, o1, log_n, log_q);
+  }
+  int32_t quotient() {
+    const gl::e2 alpha = challenge2();
+    uint32_t n_gate_terms = 0;
+    for (const auto& g : setup.gates) n_gate_terms += g.n_writes * g.num_repetitions;
+    const uint32_t n_lk_terms = lk ? nsub + 1 : 0;  // lookup terms come first (prover.rs:608-625)
+    const uint32_t total_terms = n_lk_terms + n_gate_terms + 1 + 1 + n_partial;
+    std::vector<uint64_t> powers(2 * (size_t)total_terms);
+    gl::e2 cur{1, 0};
+    for (uint32_t i = 0; i < total_terms; i++) {
+      powers[2 * i] = cur.c0;
+      powers[2 * i + 1] = cur.c1;
+      cur = gl::e2_mul(cur, alpha);
+    }
+    DevMem qq, qloc;  // qq: [2][nQ] global (c0 then c1); qloc: this rank's cosets among the first Q
+    BJ_TRY(qq.alloc(ctx, 2 * nQ));
+    uint64_t* q0 = (uint64_t*)qq.p;
+    uint64_t* q1 = q0 + nQ;
+    uint64_t* const gq0 = q0;
+    uint64_t* const gq1 = q1;
+    if (world > 1) {
+      BJ_TRY(qloc.alloc(ctx, 2 * std::max<u64>(nQl, 1)));
+      q0 = (uint64_t*)qloc.p;
+      q1 = q0 + nQl;
+      BJ_CUDA(ctx, cudaMemsetAsync(qloc.p, 0, sizeof(u64) * 2 * std::max<u64>(nQl, 1), ctx->stream));
+    } else {
+      BJ_CUDA(ctx, cudaMemsetAsync(qq.p, 0, sizeof(u64) * 2 * nQ, ctx->stream));
+    }
+    if (setup.cols.keeps_quotient_cosets()) {
+      const uint64_t* zn = (const uint64_t*)z_next.p;
+      if (nQl)
+        BJ_TRY(quotient_terms({setup.cols.tree.cols.data(), witness.tree.cols.data(), stage2.tree.cols.data(), zn, zn ? zn + nD : nullptr}, powers,
+                              n_lk_terms, n_gate_terms, nQl, q0, q1));
+    } else {
+      // one local quotient unit k at a time (global unit u: coset u on one GPU or a coset shard, a row block of ub rows of
+      // coset u / B on a split shard or on one GPU with 2^rb row blocks per coset), under the window of unit u among the units
+      // of the factor-D domain; each column set gives its columns on the unit (ColumnSet::quotient_unit), and on a row block
+      // the unit's z(omega x) columns go to the scratch too.  The unit's quotient values land in its slot [k ub, (k + 1) ub)
+      // of the local quotient cosets.
+      CosetShard shard = ctx->shard;
+      shard.log_split += setup.log_blocks;  // one GPU: every one of the Q * 2^rb units is local, global unit k = k
+      const uint32_t usplit = shard.log_split;
+      const u64 ub = n >> usplit;
+      DevMem ev;
+      BJ_TRY(ev.alloc(ctx, (size_t)(setup.cols.size() + witness.size() + n_s2 + (usplit ? 2 : 0)) * ub));
+      std::vector<const uint64_t*> sc, wc, s2c;
+      for (u64 k = 0; k < shard.local_units(Q); k++) {
+        ShardWindow window(ctx, log_d + usplit, (u32)shard.global_unit(k), usplit);
+        uint64_t* e = (uint64_t*)ev.p;
+        BJ_TRY(setup.cols.quotient_unit(ctx, shard, k, e, sc));
+        BJ_TRY(witness.quotient_unit(ctx, shard, k, e, wc));
+        BJ_TRY(stage2.quotient_unit(ctx, shard, k, e, s2c));
+        const uint64_t *z0 = nullptr, *z1 = nullptr;
+        if (usplit) {
+          BJ_TRY(bj_lde_next_row(ctx, (const uint64_t*)st2.p, n, e, log_n, log_d, 2, 0));
+          z0 = e;
+          z1 = e + ub;
+        }
+        BJ_TRY(quotient_terms({sc.data(), wc.data(), s2c.data(), z0, z1}, powers, n_lk_terms, n_gate_terms, ub, q0 + (size_t)k * ub, q1 + (size_t)k * ub));
+      }
+    }
+    z_next.release();
+    if (world > 1) {
+      // the one bulk exchange: the quotient cosets recombine (they are interpolated together at size n * Q).  Every rank sends
+      // `per` = ceil(Q * B / world) unit slots of nb = n / B rows (c0 | c1 per slot; ranks beyond the Q * B units send
+      // padding), one all-gather, then the slots are scattered to their global unit positions.
+      const u64 q_units = (u64)Q << split;
+      const u64 per = std::max<u64>(1, q_units / world);
+      DevMem snd, rcv;
+      BJ_TRY(snd.alloc(ctx, per * 2 * nb));
+      BJ_TRY(rcv.alloc(ctx, (u64)world * per * 2 * nb));
+      BJ_CUDA(ctx, cudaMemsetAsync(snd.p, 0, sizeof(u64) * per * 2 * nb, ctx->stream));
+      const u64 q_loc = ctx->shard.local_units(Q);
+      for (u64 k = 0; k < q_loc; k++) {
+        BJ_CUDA(ctx, cudaMemcpyAsync(snd.p + (2 * k) * nb, q0 + k * nb, sizeof(u64) * nb, cudaMemcpyDeviceToDevice, ctx->stream));
+        BJ_CUDA(ctx, cudaMemcpyAsync(snd.p + (2 * k + 1) * nb, q1 + k * nb, sizeof(u64) * nb, cudaMemcpyDeviceToDevice, ctx->stream));
+      }
+      BJ_TRY(comm_all_gather(ctx->comm, snd.p, rcv.p, per * 2 * nb));
+      for (uint32_t r = 0; r < world; r++)
+        for (u64 k = 0; k < per; k++) {
+          const u64 u = ctx->shard.unit_of(r, k);
+          if (u >= q_units) continue;
+          const u64* part = rcv.p + ((u64)r * per + k) * 2 * nb;
+          BJ_CUDA(ctx, cudaMemcpyAsync(gq0 + u * nb, part, sizeof(u64) * nb, cudaMemcpyDeviceToDevice, ctx->stream));
+          BJ_CUDA(ctx, cudaMemcpyAsync(gq1 + u * nb, part + nb, sizeof(u64) * nb, cudaMemcpyDeviceToDevice, ctx->stream));
+        }
+      q0 = gq0;
+      q1 = gq1;
+      qloc.release();
+    }
+    // cosets -> natural order, one interpolation of size n*Q on the coset 7, Q chunks of n coefficients (prover.rs:1399-1467)
+    BJ_TRY(bj_bitreverse(ctx, q0, log_n + log_q, 2, nQ));
+    BJ_TRY(bj_intt_natural_to_natural(ctx, q0, log_n + log_q, 2, nQ, gl::MULT_GEN));
+    {
+      // the reference's satisfiability guard: the top coefficient must vanish (prover.rs:1425-1438)
+      uint64_t top[2];
+      BJ_CUDA(ctx, cudaMemcpyAsync(&top[0], q0 + nQ - 1, sizeof(u64), cudaMemcpyDeviceToHost, ctx->stream));
+      BJ_CUDA(ctx, cudaMemcpyAsync(&top[1], q1 + nQ - 1, sizeof(u64), cudaMemcpyDeviceToHost, ctx->stream));
+      BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+      if (top[0] || top[1]) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: unsatisfied circuit (quotient is not a polynomial of degree < n * quotient_degree)");
+    }
+    DevMem chunks;  // chunk j: c0 then c1
+    BJ_TRY(chunks.alloc(ctx, 2 * nQ));
+    for (uint32_t j = 0; j < Q; j++) {
+      BJ_CUDA(ctx, cudaMemcpyAsync(chunks.p + (size_t)(2 * j) * n, q0 + (size_t)j * n, sizeof(u64) * n, cudaMemcpyDeviceToDevice, ctx->stream));
+      BJ_CUDA(ctx, cudaMemcpyAsync(chunks.p + (size_t)(2 * j + 1) * n, q1 + (size_t)j * n, sizeof(u64) * n, cudaMemcpyDeviceToDevice, ctx->stream));
+    }
+    qq.release();
+    BJ_TRY(qt_lde.alloc(ctx, (size_t)(2 * Q) * nL));
+    BJ_TRY(bj_lde(ctx, (const uint64_t*)chunks.p, n, (uint64_t*)qt_lde.p, log_n, log_l, 2 * Q, 1));
+    chunks.release();
+    for (uint32_t j = 0; j < 2 * Q; j++) qt.cols.push_back((const uint64_t*)qt_lde.p + (size_t)j * nL);
+    BJ_TRY(oracle_build(ctx, qt, n << log_l, cap, c.tree_hasher, L));
+    pf.quotient_cap = qt.cap;
+    bj_transcript_witness_merkle_tree_cap(tr, (const uint64_t*)qt.cap.data(), cap);
+    return BJ_OK;
+  }
+
+  // chunks of `chunk` rebuilt columns among flat [lo, hi) (an Fp2 pair never split; a chunk may span two oracles): monomials
+  // by one iNTT, then body(c0, cnt, monomials, scratch for one unit of the chunk: a coset, or nb rows of one on a split shard,
+  // stride nb)
+  int32_t for_chunks(uint32_t lo, uint32_t hi, const std::function<int32_t(uint32_t, uint32_t, const uint64_t*, uint64_t*)>& body) {
+    DevMem mono, ev;
+    BJ_TRY(mono.alloc(ctx, (size_t)setup.chunk * n));
+    BJ_TRY(ev.alloc(ctx, (size_t)setup.chunk * nb));
+    for (uint32_t c0 = lo; c0 < hi;) {
+      uint32_t cnt = std::min<uint32_t>(setup.chunk, hi - c0);
+      if (c0 + cnt < hi && pair_start(c0 + cnt - 1)) cnt--;
+      std::vector<const uint64_t*> nat;
+      for_flat(c0, c0 + cnt, [&](uint32_t o, uint32_t j, uint32_t) { nat.push_back(set(o).nat_col(j)); });
+      for (uint32_t i = 0; i < cnt; i++)
+        BJ_CUDA(ctx, cudaMemcpyAsync(mono.p + (size_t)i * n, nat[i], sizeof(u64) * n, cudaMemcpyDeviceToDevice, ctx->stream));
+      BJ_TRY(bj_intt_natural_to_natural(ctx, (uint64_t*)mono.p, log_n, cnt, n, 1));
+      BJ_TRY(body(c0, cnt, (const uint64_t*)mono.p, (uint64_t*)ev.p));
+      c0 += cnt;
+    }
+    return BJ_OK;
+  }
+
+  // ---- round 4: openings.  Order (prover.rs:1549-1683): variables, witness, constants, sigmas, z, partial products,
+  //      multiplicities, lookup A, lookup B, lookup tables, quotient chunks.
+  // The barycentric sums of `cols` (oracle, column) at a into ev.  On the recompute plan the setup, witness and stage-2
+  // columns come from local slot 0 (coset 0 on one GPU, this rank's coset or row block on a sharded context), rebuilt a chunk
+  // at a time (only the chunks that hold one of them); the quotient oracle's columns are read directly.
+  int32_t barycentric(const std::vector<std::pair<uint32_t, uint32_t>>& cols, const uint64_t a[2], uint64_t* ev) {
+    auto evaluate = [&](const std::vector<const uint64_t*>& ptrs, const std::vector<size_t>& at) -> int32_t {
+      if (ptrs.empty()) return BJ_OK;
+      std::vector<uint64_t> got(2 * ptrs.size());
+      BJ_TRY(bj_barycentric_evaluate(ctx, ptrs.data(), (uint32_t)ptrs.size(), log_n, a, got.data()));
+      for (size_t k = 0; k < at.size(); k++) {
+        ev[2 * at[k]] = got[2 * k];
+        ev[2 * at[k] + 1] = got[2 * k + 1];
+      }
+      return BJ_OK;
+    };
+    std::vector<const uint64_t*> direct;
+    std::vector<size_t> direct_at;
+    uint32_t lo = n_rebuilt, hi = 0;
+    const bool rebuilt = setup.plan == PLAN_RECOMPUTE;  // on coset 0 of the rebuilt columns
+    for (size_t i = 0; i < cols.size(); i++) {
+      const auto [o, j] = cols[i];
+      if (!rebuilt || o == QUOTIENT) {
+        direct.push_back(col(o, j));
+        direct_at.push_back(i);
+      } else {
+        lo = std::min(lo, base[o] + j);
+        hi = std::max(hi, base[o] + j + 1);
+      }
+    }
+    BJ_TRY(evaluate(direct, direct_at));
+    if (!rebuilt) return BJ_OK;
+    return for_chunks(lo, hi, [&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* on_coset) -> int32_t {
+      BJ_TRY(lde_unit(ctx, mono, on_coset, log_n, log_l, cnt, 0, 1));
+      std::vector<const uint64_t*> ptrs;
+      std::vector<size_t> at;
+      for (size_t i = 0; i < cols.size(); i++) {
+        const auto [o, j] = cols[i];
+        if (o == QUOTIENT || base[o] + j < c0 || base[o] + j >= c0 + cnt) continue;
+        ptrs.push_back(on_coset + (size_t)(base[o] + j - c0) * nb);
+        at.push_back(i);
+      }
+      return evaluate(ptrs, at);
+    });
+  }
+  int32_t open_at(const std::vector<Src>& srcs, gl::e2 at, std::vector<gl::e2>& vals) {
+    std::vector<std::pair<uint32_t, uint32_t>> flat;
+    for (const auto& s : srcs) {
+      flat.push_back({s.oracle, s.col});
+      if (s.ext) flat.push_back({s.oracle, s.col + 1});
+    }
+    vals.clear();
+    if (flat.empty()) return BJ_OK;
+    std::vector<uint64_t> ev(2 * flat.size());
+    const uint64_t a[2] = {at.c0, at.c1};
+    if (world == 1) {
+      BJ_TRY(barycentric(flat, a, ev.data()));
+    } else {
+      // the columns are split over the coset groups: ranks [g B, (g + 1) B) hold the B row blocks of coset g (B = 1: one rank,
+      // its whole coset) and open column block g from it, each rank its block's contribution (on the recompute plan from its
+      // rebuilt local slot 0).  The contributions are gathered and the B of a group summed.
+      const uint32_t groups = world >> split, g = rank >> split;
+      const size_t per = (flat.size() + groups - 1) / groups, first = std::min(flat.size(), (size_t)g * per);
+      const size_t cnt = std::min(per, flat.size() - first);
+      std::vector<uint64_t> mine(2 * per, 0), all(2 * per * world);
+      if (cnt) BJ_TRY(barycentric(std::vector<std::pair<uint32_t, uint32_t>>(flat.begin() + first, flat.begin() + first + cnt), a, mine.data()));
+      BJ_TRY(comm_all_gather_host(ctx->comm, (const u64*)mine.data(), (u64*)all.data(), 2 * per));
+      for (uint32_t gg = 0; gg < groups; gg++)
+        for (size_t e = 0; e < 2 * per && gg * 2 * per + e < ev.size(); e++) {
+          u64 v = 0;
+          for (uint32_t p = 0; p < (1u << split); p++) v = gl::canon(gl::add(v, all[(((size_t)gg << split) + p) * 2 * per + e]));
+          ev[gg * 2 * per + e] = v;  // group blocks are contiguous: [g][per] == flat order
+        }
+    }
+    size_t k = 0;
+    for (const auto& s : srcs) {
+      if (s.ext) {  // f0 + u f1 at an Fp2 point (u^2 = 7)
+        const gl::e2 a0{ev[2 * k], ev[2 * k + 1]}, b0{ev[2 * k + 2], ev[2 * k + 3]};
+        vals.push_back({gl::canon(gl::add(a0.c0, gl::mul7(b0.c1))), gl::canon(gl::add(a0.c1, b0.c0))});
+        k += 2;
+      } else {
+        vals.push_back({ev[2 * k], ev[2 * k + 1]});
+        k += 1;
+      }
+    }
+    return BJ_OK;
+  }
+  int32_t openings() {
+    z = challenge2();
+    z_omega = gl::e2_mul_base(z, gl::omega(log_n));
+    for (uint32_t j = 0; j < V; j++) sources.push_back({WITNESS, j, false});
+    for (uint32_t j = 0; j < C; j++) sources.push_back({SETUP, V + j, false});
+    for (uint32_t j = 0; j < V; j++) sources.push_back({SETUP, j, false});
+    for (uint32_t i = 0; i < 1 + n_partial; i++) sources.push_back({STAGE2, 2 * i, true});
+    if (lk) {
+      sources.push_back({WITNESS, V, false});
+      for (uint32_t i = 0; i < nsub + 1; i++) {
+        sources.push_back({STAGE2, a_off + 2 * i, true});
+        zero_sources.push_back({STAGE2, a_off + 2 * i, true});
+      }
+      for (uint32_t j = 0; j < T; j++) sources.push_back({SETUP, V + C + j, false});
+    }
+    for (uint32_t i = 0; i < Q; i++) sources.push_back({QUOTIENT, 2 * i, true});
+    z_omega_sources = {{STAGE2, 0, true}};
+    BJ_TRY(open_at(sources, z, pf.values_at_z));
+    BJ_TRY(open_at(z_omega_sources, z_omega, pf.values_at_z_omega));
+    BJ_TRY(open_at(zero_sources, gl::e2{0, 0}, pf.values_at_0));
+    for (const auto* vs : {&pf.values_at_z, &pf.values_at_z_omega, &pf.values_at_0})
+      for (const auto& v : *vs) {
+        const uint64_t e[2] = {v.c0, v.c1};
+        bj_transcript_witness_field_elements(tr, e, 2);
+      }
+    return BJ_OK;
+  }
+
+  // ---- round 5: DEEP combination + FRI ----
+  struct DeepGroup {
+    const std::vector<Src>* srcs;
+    const std::vector<gl::e2>* vals;
+    gl::e2 at;
+    const uint64_t* chs;
+  };
+  // sources i of a group with keep(i) on the local points [first, first + count), column j of oracle o read at at_col(o, j).
+  // One GPU: any run of points.  Sharded (recompute plan): the whole local domain, or local unit k (first = k nb, count = nb)
+  // under its window, whose points the kernel then places at their global indices.
+  int32_t deep_range(const DeepGroup& g, const std::function<bool(size_t)>& keep, const std::function<const uint64_t*(uint32_t, uint32_t)>& at_col,
+                     u64 first, u64 count) {
+    std::vector<const uint64_t*> p0, p1;
+    std::vector<uint64_t> v, ch;
+    for (size_t i = 0; i < g.srcs->size(); i++) {
+      if (!keep(i)) continue;
+      const Src& sr = (*g.srcs)[i];
+      p0.push_back(at_col(sr.oracle, sr.col));
+      p1.push_back(sr.ext ? at_col(sr.oracle, sr.col + 1) : nullptr);
+      v.push_back((*g.vals)[i].c0);
+      v.push_back((*g.vals)[i].c1);
+      ch.push_back(g.chs[2 * i]);
+      ch.push_back(g.chs[2 * i + 1]);
+    }
+    if (p0.empty()) return BJ_OK;
+    const uint64_t a[2] = {g.at.c0, g.at.c1};
+    uint64_t *acc0 = (uint64_t*)deep.p + first, *acc1 = (uint64_t*)deep.p + nL + first;
+    if (world == 1)
+      return bj_deep_quotient_range(ctx, p0.data(), p1.data(), (uint32_t)p0.size(), v.data(), ch.data(), a, log_n + log_l, first, count, acc0, acc1);
+    if (count == nL)
+      return bj_deep_quotient_group(ctx, p0.data(), p1.data(), (uint32_t)p0.size(), v.data(), ch.data(), a, log_n + log_l, acc0, acc1);
+    ShardWindow window(ctx, log_l + split, (u32)ctx->shard.global_unit(first / nb), split);
+    return bj_deep_quotient_group(ctx, p0.data(), p1.data(), (uint32_t)p0.size(), v.data(), ch.data(), a, log_n + log_l, acc0, acc1);
+  }
+  int32_t deep_fri_pow() {
+    // public inputs grouped by opening point w^row in order of first appearance (prover.rs:1805-1821)
+    struct PiGroup {
+      u64 at;
+      std::vector<Src> srcs;
+      std::vector<gl::e2> vals;
+    };
+    std::vector<PiGroup> pi_groups;
+    for (uint32_t i = 0; i < c.n_public_inputs; i++) {
+      const u64 at = gl::pow(gl::omega(log_n), setup.pi_rows[i]);
+      PiGroup* g = nullptr;
+      for (auto& e : pi_groups)
+        if (e.at == at) g = &e;
+      if (!g) {
+        pi_groups.push_back({at, {}, {}});
+        g = &pi_groups.back();
+      }
+      g->srcs.push_back({WITNESS, setup.pi_cols[i], false});
+      g->vals.push_back({pf.public_inputs[i], 0});
+    }
+    const gl::e2 ch0 = challenge2();
+    const size_t n_ch = pf.values_at_z.size() + 1 + pf.values_at_0.size() + c.n_public_inputs;
+    std::vector<uint64_t> ch(2 * n_ch);
+    gl::e2 cur{1, 0};
+    for (size_t i = 0; i < n_ch; i++) {
+      ch[2 * i] = cur.c0;
+      ch[2 * i + 1] = cur.c1;
+      cur = gl::e2_mul(cur, ch0);
+    }
+    BJ_TRY(deep.alloc(ctx, 2 * nL));
+    BJ_CUDA(ctx, cudaMemsetAsync(deep.p, 0, sizeof(u64) * 2 * nL, ctx->stream));
+    // with units rebuilt: units [0, first_rebuilt) from the kept columns, the quotient oracle's columns on all local units,
+    // the rest added below
+    const u64 Fn = rebuild ? first_rebuilt * n : 0;
+    std::vector<DeepGroup> deep_groups;
+    auto deep_group = [&](const std::vector<Src>& srcs, const std::vector<gl::e2>& vals, gl::e2 at, const uint64_t* chs) -> int32_t {
+      if (srcs.empty()) return BJ_OK;
+      const DeepGroup g{&srcs, &vals, at, chs};
+      if (rebuild) {
+        deep_groups.push_back(g);
+        if (Fn) BJ_TRY(deep_range(g, [](size_t) { return true; }, [&](uint32_t o, uint32_t j) { return col(o, j); }, 0, Fn));
+        return deep_range(g, [&](size_t i) { return srcs[i].oracle == QUOTIENT; }, [&](uint32_t o, uint32_t j) { return col(o, j) + Fn; }, Fn, nL - Fn);
+      }
+      std::vector<const uint64_t*> p0(srcs.size()), p1(srcs.size());
+      std::vector<uint64_t> v(2 * srcs.size());
+      for (size_t i = 0; i < srcs.size(); i++) {
+        p0[i] = col(srcs[i].oracle, srcs[i].col);
+        p1[i] = srcs[i].ext ? col(srcs[i].oracle, srcs[i].col + 1) : nullptr;
+        v[2 * i] = vals[i].c0;
+        v[2 * i + 1] = vals[i].c1;
+      }
+      const uint64_t a[2] = {at.c0, at.c1};
+      return bj_deep_quotient_group(ctx, p0.data(), p1.data(), (uint32_t)srcs.size(), v.data(), chs, a, log_n + log_l /* global */,
+                                    (uint64_t*)deep.p, (uint64_t*)deep.p + nL);
+    };
+    BJ_TRY(deep_group(sources, pf.values_at_z, z, ch.data()));
+    BJ_TRY(deep_group(z_omega_sources, pf.values_at_z_omega, z_omega, ch.data() + 2 * sources.size()));
+    BJ_TRY(deep_group(zero_sources, pf.values_at_0, gl::e2{0, 0}, ch.data() + 2 * (sources.size() + 1)));
+    size_t off = sources.size() + 1 + zero_sources.size();
+    for (const auto& g : pi_groups) {  // prover.rs:2010-2041
+      BJ_TRY(deep_group(g.srcs, g.vals, gl::e2{g.at, 0}, ch.data() + 2 * off));
+      off += g.srcs.size();
+    }
+    if (rebuild)  // units [first_rebuilt, units_l): every chunk of natural columns evaluated on one unit at a time, its DEEP terms added
+      BJ_TRY(for_chunks(0, n_rebuilt, [&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* ev) -> int32_t {
+        auto in_chunk = [&](const Src& s) { return s.oracle != QUOTIENT && base[s.oracle] + s.col >= c0 && base[s.oracle] + s.col < c0 + cnt; };
+        auto on_unit = [&](uint32_t o, uint32_t j) -> const uint64_t* { return ev + (size_t)(base[o] + j - c0) * nb; };
+        for (u64 k = first_rebuilt; k < units_l; k++) {
+          BJ_TRY(lde_unit(ctx, mono, ev, log_n, log_l, cnt, k, 1));
+          for (const DeepGroup& g : deep_groups) BJ_TRY(deep_range(g, [&](size_t i) { return in_chunk((*g.srcs)[i]); }, on_unit, k * nb, nb));
+        }
+        return BJ_OK;
+      }));
+    uint32_t new_pow = 0, final_degree = 0;
+    BJ_TRY(bj_compute_fri_schedule(c.security_level, cap, c.pow_bits, log_l, log_n, &new_pow, &num_queries, sched, &sched_len, &final_degree));
+    BJ_TRY(bj_do_fri_with_hasher(ctx, tr, (const uint64_t*)deep.p, (const uint64_t*)deep.p + nL, log_n + log_l, sched, sched_len, log_l, cap,
+                                 c.tree_hasher, &fri));
+    const uint32_t n_fri = bj_fri_oracles_num_oracles(fri);
+    pf.fri_caps.resize(n_fri);
+    for (uint32_t i = 0; i < n_fri; i++) {
+      pf.fri_caps[i].resize(4 * (size_t)cap);
+      BJ_TRY(bj_fri_oracles_get_cap(fri, i, (uint64_t*)pf.fri_caps[i].data()));
+    }
+    const uint32_t n_mono = bj_fri_oracles_num_monomials(fri);
+    pf.mono_c0.resize(n_mono);
+    pf.mono_c1.resize(n_mono);
+    BJ_TRY(bj_fri_oracles_get_monomials(fri, (uint64_t*)pf.mono_c0.data(), (uint64_t*)pf.mono_c1.data()));
+    if (new_pow) {  // prover.rs:2109-2132 with POW = Blake2s256: 5 challenges seed the search, the nonce re-enters the transcript
+      uint8_t seed[40];
+      for (int i = 0; i < 5; i++) {
+        const uint64_t e = bj_transcript_get_challenge(tr);
+        for (int k = 0; k < 8; k++) seed[8 * i + k] = (uint8_t)(e >> (8 * k));
+      }
+      uint64_t nonce = 0;
+      BJ_TRY(bj_pow_blake2s(ctx, seed, 40, new_pow, &nonce));
+      pf.pow_challenge = nonce;
+      const uint64_t lh[2] = {nonce & 0xffffffffull, nonce >> 32};
+      bj_transcript_witness_field_elements(tr, lh, 2);
+    }
+    return BJ_OK;
+  }
+
+  // ---- queries ----
+  int32_t queries() {
+    const uint32_t max_bits = log_n + log_l;
+    std::vector<uint64_t> idxs(num_queries);
+    for (auto& i : idxs) i = bj_transcript_get_index_bits(tr, max_bits, max_bits);
+    pf.queries.assign(num_queries, {});
+    // a query is answered by the rank that owns the unit of its index (leaf t = coset * n + row lies in that rank's subtree);
+    // the other ranks look up a dummy leaf, the answers are exchanged and every rank keeps the owner's
+    std::vector<uint64_t> loc_idx(num_queries);
+    std::vector<uint32_t> owner(num_queries);
+    for (uint32_t q = 0; q < num_queries; q++) {
+      owner[q] = ctx->shard.owner(idxs[q], (int)log_n);
+      loc_idx[q] = owner[q] == rank ? ctx->shard.owner_index(idxs[q], (int)log_n) : 0;
+    }
+    // every answer part (leaf elements / path of one oracle) is gathered locally first; ONE exchange then carries all of them
+    struct Part {
+      std::vector<uint64_t> data;  // [num_queries][rec_len]
+      size_t rec_len;
+    };
+    std::vector<Part> parts;  // order: (rows, path) of the 4 base oracles (OracleId order), then (leaf elements, path) of every FRI level
+    const u64 Fn = rebuild ? first_rebuilt * n : 0;
+    for (uint32_t oi : {WITNESS, STAGE2, QUOTIENT, SETUP}) {
+      const Oracle* o = &oracle(oi);
+      const size_t row_len = o->cols.size();
+      uint32_t depth = 0;
+      while ((o->n_leaves >> depth) > o->cap_size) depth++;
+      Part rows{std::vector<uint64_t>((size_t)num_queries * row_len), row_len};
+      Part path{std::vector<uint64_t>((size_t)num_queries * depth * 4), (size_t)depth * 4};
+      if (!rebuild || oi == QUOTIENT) {
+        BJ_TRY(bj_query_leaf_elements(ctx, o->cols.data(), (uint32_t)row_len, 1, o->n_leaves, loc_idx.data(), num_queries, rows.data.data()));
+      } else if (Fn) {  // kept columns hold the first units; the rows of the others are recomputed below
+        std::vector<uint64_t> kept_idx(loc_idx);
+        for (auto& i : kept_idx)
+          if (i >= Fn) i = 0;
+        BJ_TRY(bj_query_leaf_elements(ctx, o->cols.data(), (uint32_t)row_len, 1, Fn, kept_idx.data(), num_queries, rows.data.data()));
+      }
+      if (depth)
+        BJ_TRY(bj_merkle_paths(ctx, (const uint64_t*)o->leaf_hashes.p, (const uint64_t*)o->nodes.p, o->n_leaves, o->cap_size, loc_idx.data(),
+                               num_queries, path.data.data()));
+      parts.push_back(std::move(rows));
+      parts.push_back(std::move(path));
+    }
+    if (rebuild) {
+      // queries this context answers whose leaf lies in a local unit k >= first_rebuilt (a coset on one GPU): one recompute of
+      // each such unit per chunk, the queried rows gathered from it (the rows of every query, so that the gather buffer is the
+      // one the plan counts) into the rows part of each column's oracle.  On a sharded context every rank runs the pass, also
+      // one that answers none of these queries: its peers are rebuilding meanwhile and the exchange waits for them, so it
+      // gathers from the chunk's monomials instead, and every rank's pool reaches the peak its plan counts.
+      const u32 log_nb = log_n - split;
+      std::vector<std::vector<uint32_t>> by_unit(units_l);
+      for (uint32_t q = 0; q < num_queries; q++)
+        if (owner[q] == rank && (loc_idx[q] >> log_nb) >= first_rebuilt) by_unit[loc_idx[q] >> log_nb].push_back(q);
+      bool any = false;
+      for (const auto& qs : by_unit) any = any || !qs.empty();
+      if (any || world > 1)
+        BJ_TRY(for_chunks(0, n_rebuilt, [&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* ev) -> int32_t {
+          std::vector<const uint64_t*> cols(cnt);
+          std::vector<uint64_t> rows_in(num_queries, 0), got((size_t)num_queries * cnt);
+          if (!any) {
+            for (uint32_t i = 0; i < cnt; i++) cols[i] = mono + (size_t)i * n;
+            return bj_query_leaf_elements(ctx, cols.data(), cnt, 1, n, rows_in.data(), num_queries, got.data());
+          }
+          for (uint32_t i = 0; i < cnt; i++) cols[i] = ev + (size_t)i * nb;
+          for (u64 k = first_rebuilt; k < units_l; k++) {
+            const auto& qs = by_unit[k];
+            if (qs.empty()) continue;
+            BJ_TRY(lde_unit(ctx, mono, ev, log_n, log_l, cnt, k, 1));
+            for (uint32_t q : qs) rows_in[q] = loc_idx[q] & (nb - 1);
+            BJ_TRY(bj_query_leaf_elements(ctx, cols.data(), cnt, 1, nb, rows_in.data(), num_queries, got.data()));
+            for_flat(c0, c0 + cnt, [&](uint32_t o, uint32_t j, uint32_t i) {
+              Part& pt = parts[2 * o];
+              for (uint32_t q : qs) pt.data[(size_t)q * pt.rec_len + j] = got[(size_t)q * cnt + (i - c0)];
+            });
+          }
+          return BJ_OK;
+        }));
+    }
+    uint32_t log_len = log_n;  // coset length of the level's codeword
+    std::vector<uint64_t> sub(idxs);
+    for (uint32_t lvl = 0; lvl < sched_len; lvl++) {
+      const uint32_t k = sched[lvl];
+      const size_t le_len = (size_t)2 << k;
+      std::vector<uint64_t> locals(num_queries);
+      for (uint32_t q = 0; q < num_queries; q++) {
+        locals[q] = owner[q] == rank ? (ctx->shard.owner_index(sub[q], (int)log_len) >> k) : 0;
+        sub[q] >>= k;
+      }
+      uint32_t plen = 0;
+      Part les{std::vector<uint64_t>((size_t)num_queries * le_len, 0), le_len};
+      Part path{std::vector<uint64_t>((size_t)num_queries * 40 * 4, 0), 0};  // [num_queries][plen][4] after the call
+      BJ_TRY(bj_fri_oracles_query_batch(fri, lvl, locals.data(), num_queries, les.data.data(), path.data.data(), &plen));
+      path.rec_len = (size_t)plen * 4;
+      path.data.resize((size_t)num_queries * path.rec_len);
+      parts.push_back(std::move(les));
+      parts.push_back(std::move(path));
+      log_len -= k;
+    }
+    if (world > 1) {
+      size_t total = 0;
+      for (const auto& pt : parts) total += pt.data.size();
+      std::vector<uint64_t> mine(total), all((size_t)world * total);
+      size_t off = 0;
+      for (const auto& pt : parts) {
+        if (!pt.data.empty()) memcpy(mine.data() + off, pt.data.data(), sizeof(uint64_t) * pt.data.size());
+        off += pt.data.size();
+      }
+      BJ_TRY(comm_all_gather_host(ctx->comm, (const u64*)mine.data(), (u64*)all.data(), total));
+      off = 0;
+      for (auto& pt : parts) {
+        for (uint32_t q = 0; q < num_queries && pt.rec_len; q++)
+          memcpy(pt.data.data() + (size_t)q * pt.rec_len, all.data() + (size_t)owner[q] * total + off + (size_t)q * pt.rec_len,
+                 sizeof(uint64_t) * pt.rec_len);
+        off += pt.data.size();
+      }
+    }
+    for (size_t o = 0; o + 1 < parts.size(); o += 2) {
+      const Part &le = parts[o], &pa = parts[o + 1];
+      for (uint32_t q = 0; q < num_queries; q++) {
+        QueryAnswer a;
+        a.leaf_elements.assign(le.data.begin() + (size_t)q * le.rec_len, le.data.begin() + (size_t)(q + 1) * le.rec_len);
+        a.path.assign(pa.data.begin() + (size_t)q * pa.rec_len, pa.data.begin() + (size_t)(q + 1) * pa.rec_len);
+        pf.queries[q].push_back(std::move(a));
+      }
+    }
+    return BJ_OK;
+  }
+};
+
+// ---- serde_json shape of Proof (proof.rs:57-143) ----
+static std::string proof_json(const bj_proof& pf, uint32_t sched_len) {
+  const bj_circuit& c = pf.c;
+  const uint32_t cap = c.merkle_tree_cap_size;
+  std::string s;
+  s.reserve(1 << 20);
+  const bool digest_bytes = c.tree_hasher != BJ_HASHER_POSEIDON2;
+  s += "{\"proof_config\":{\"fri_lde_factor\":" + std::to_string(c.fri_lde_factor) + ",\"merkle_tree_cap_size\":" + std::to_string(cap) +
+       ",\"fri_folding_schedule\":null,\"security_level\":" + std::to_string(c.security_level) + ",\"pow_bits\":" + std::to_string(c.pow_bits) +
+       "},\"public_inputs\":";
+  json_u64_list(s, pf.public_inputs.data(), pf.public_inputs.size());
+  s += ",\"witness_oracle_cap\":";
+  json_digests(s, pf.witness_cap.data(), cap, digest_bytes);
+  s += ",\"stage_2_oracle_cap\":";
+  json_digests(s, pf.stage2_cap.data(), cap, digest_bytes);
+  s += ",\"quotient_oracle_cap\":";
+  json_digests(s, pf.quotient_cap.data(), cap, digest_bytes);
+  s += ",\"final_fri_monomials\":[";
+  json_u64_list(s, pf.mono_c0.data(), pf.mono_c0.size());
+  s += ',';
+  json_u64_list(s, pf.mono_c1.data(), pf.mono_c1.size());
+  s += "],\"values_at_z\":";
+  json_ext_list(s, pf.values_at_z);
+  s += ",\"values_at_z_omega\":";
+  json_ext_list(s, pf.values_at_z_omega);
+  s += ",\"values_at_0\":";
+  json_ext_list(s, pf.values_at_0);
+  s += ",\"fri_base_oracle_cap\":";
+  json_digests(s, pf.fri_caps[0].data(), cap, digest_bytes);
+  s += ",\"fri_intermediate_oracles_caps\":[";
+  for (size_t i = 1; i < pf.fri_caps.size(); i++) {
+    if (i > 1) s += ',';
+    json_digests(s, pf.fri_caps[i].data(), cap, digest_bytes);
+  }
+  s += "],\"queries_per_fri_repetition\":[";
+  static const char* names[4] = {"witness_query", "stage_2_query", "quotient_query", "setup_query"};
+  auto json_answer = [&](const QueryAnswer& a) {
+    s += "{\"leaf_elements\":";
+    json_u64_list(s, a.leaf_elements.data(), a.leaf_elements.size());
+    s += ",\"proof\":";
+    json_digests(s, a.path.data(), a.path.size() / 4, digest_bytes);
+    s += '}';
+  };
+  for (size_t q = 0; q < pf.queries.size(); q++) {
+    if (q) s += ',';
+    s += '{';
+    for (int o = 0; o < 4; o++) {
+      s += std::string("\"") + names[o] + "\":";
+      json_answer(pf.queries[q][o]);
+      s += ',';
+    }
+    s += "\"fri_queries\":[";
+    for (uint32_t lvl = 0; lvl < sched_len; lvl++) {
+      if (lvl) s += ',';
+      json_answer(pf.queries[q][4 + lvl]);
+    }
+    s += "]}";
+  }
+  s += "],\"pow_challenge\":" + std::to_string(pf.pow_challenge) + ",\"_marker\":null}";
+  return s;
 }
 
 extern "C" {
@@ -749,106 +1692,7 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
     *out = s.release();
     return BJ_OK;
   };
-  {
-    // the memory plan: resident if it fits under the limit, else compact (Q < L, one GPU), else streamed (Q > L), else
-    // recompute (one GPU when the context allows it, a context with a communicator when it allows the sharded recompute
-    // plan); refused before anything is launched.  On a sharded context every rank chooses under its own limit: every plan
-    // commits to the same units and runs the same collectives, so ranks on different plans still agree
-    ProofShape sh;
-    BJ_TRY(proof_shape(*circuit, comm_world(ctx), &sh));
-    s->plan[0] = plan_bytes(sh, PLAN_RESIDENT);
-    s->plan[1] = compact_applies(sh) ? plan_bytes(sh, PLAN_COMPACT) : 0;
-    s->plan[2] = streamed_applies(sh) ? plan_bytes(sh, PLAN_STREAMED) : 0;
-    const bool recompute_allowed = (ctx->allow_recompute_plan && recompute_applies(sh)) ||
-                                   (ctx->allow_sharded_recompute_plan && ctx->comm && recompute_sharded_applies(sh));
-    BJ_TRY(memory_limit(ctx, &s->limit));
-    // with lanes alive on the context, a plan must also hold their proofs: one lane part each beside the plan, and the
-    // witness slot sets alive on the lanes
-    const uint32_t lanes = ctx->lanes.load();
-    uint64_t lane_sets = 0;
-    {
-      std::lock_guard<std::mutex> lock(ctx->tables_mu);
-      lane_sets = ctx->lane_witness_set_bytes;
-    }
-    auto need_of = [&](const ProofShape& shape, MemoryPlan k) {
-      uint64_t v = plan_bytes(shape, k);
-      if (lanes) {
-        uint64_t lp[3];
-        lane_plan(shape, k, 2, 1, lp);
-        v += (uint64_t)lanes * lp[1] + lane_sets;
-      }
-      return v;
-    };
-    uint64_t need[4];
-    for (int k = 0; k < 3; k++) need[k] = s->plan[k] ? need_of(sh, (MemoryPlan)k) : 0;
-    // the recompute plan on one GPU: the fewest row blocks per coset (up to the context's bj_ctx_set_max_row_blocks) whose
-    // plan fits, or the most allowed when none does, so that a refusal names the smallest recompute plan on offer
-    uint32_t rb = 0;
-    need[3] = 0;
-    if (recompute_allowed) {
-      uint32_t max_rb = 0;
-      while (!ctx->comm && (2u << max_rb) <= ctx->max_row_blocks && row_blocks_valid(sh, max_rb + 1)) max_rb++;
-      ProofShape shb = sh;
-      for (;; rb++) {
-        shb.rb = rb;
-        need[3] = need_of(shb, PLAN_RECOMPUTE);
-        if (need[3] <= s->limit || rb == max_rb) break;
-      }
-      s->plan[3] = plan_bytes(shb, PLAN_RECOMPUTE);
-    }
-    auto fits = [&](int k) { return need[k] && need[k] <= s->limit; };
-    if (need[0] > s->limit) {
-      if (fits(2)) s->streamed = true;
-      else if (fits(1)) s->compact = true;
-      else if (fits(3)) s->recompute = true;
-      else
-        BJ_FAIL(ctx, BJ_ERR_OOM, plan_message("bj_setup_create", need, s->limit) +
-                                     (lanes ? " (each plan counted with the " + std::to_string(lanes) + " lane(s) of the context" +
-                                                  (lane_sets ? " and their witness slot sets of " + std::to_string(lane_sets) + " bytes)" : std::string(")"))
-                                            : std::string()));
-    }
-    if (ctx->comm && ctx->allow_sharded_recompute_plan && comm_world(ctx) > 1) {
-      // The resident and streamed plans share their LDEs' monomials (lde_columns: every rank interpolates a block of the
-      // columns, one all-gather per column group); the recompute plan evaluates its units from the natural-order columns and
-      // takes part in no such exchange.  So the ranks agree before their first collective: once one rank needs the recompute
-      // plan every rank takes it (a proof runs at its slowest rank's pace, so this costs the others no time), or, where a
-      // rank's limit does not hold it, every rank refuses.
-      const uint32_t world = comm_world(ctx);
-      const u64 mine[2] = {s->recompute ? 1u : 0u, fits(3) ? 1u : 0u};
-      std::vector<u64> all(2 * (size_t)world);
-      BJ_TRY(comm_all_gather_host(ctx->comm, mine, all.data(), 2));
-      bool any = false, every = true;
-      for (uint32_t r = 0; r < world; r++) {
-        any = any || all[2 * r];
-        every = every && all[2 * r + 1];
-      }
-      if (any && !every)
-        BJ_FAIL(ctx, BJ_ERR_OOM, "bj_setup_create: a rank needs the recompute plan and another rank's limit does not hold it; " +
-                                     plan_message("this rank", need, s->limit));
-      if (any) {
-        s->streamed = false;
-        s->recompute = true;
-      }
-    }
-    if (s->recompute) s->log_blocks = rb;
-    sh.rb = s->log_blocks;
-    if (s->compact || s->recompute) {
-      // wider recompute chunks only save kernel launches: the chunk grows into at most half of the headroom the limit leaves
-      // over the plan (the rest is slack for the pool's fragmentation) and stops at 16 columns
-      const MemoryPlan kind = s->compact ? PLAN_COMPACT : PLAN_RECOMPUTE;
-      const uint64_t planned = s->plan[s->compact ? 1 : 3];
-      const uint64_t budget = planned + (s->limit - planned) / 2;
-      uint32_t lo = 2, hi = std::max<uint32_t>(2, std::min<uint32_t>(16, sh.nat_cols()));
-      while (lo < hi) {
-        const uint32_t mid = lo + (hi - lo + 1) / 2;
-        if (plan_bytes(sh, kind, mid) <= budget) lo = mid;
-        else hi = mid - 1;
-      }
-      s->chunk = lo;
-    }
-    s->pool_bytes = pool_peak(sh, s->compact ? PLAN_COMPACT : s->streamed ? PLAN_STREAMED : s->recompute ? PLAN_RECOMPUTE : PLAN_RESIDENT, s->chunk);
-    s->outside_pool_bytes = library_reserve(sh);
-  }
+  BJ_TRY(choose_plan(ctx, circuit, s.get()));
   s->ctx = ctx;
   s->c = *circuit;
   // deep copy of the gate programs (the caller's arrays need not outlive this call)
@@ -881,31 +1725,14 @@ int32_t bj_setup_create(bj_ctx* ctx, const bj_circuit* circuit, const uint64_t* 
   s->tables = d_lookup_tables;
   s->n_tables = circuit->lookup_width ? circuit->lookup_width + 1 : 0;
   const uint32_t V = circuit->num_variables, C = circuit->num_constants, T = s->n_tables;
-  const uint32_t log_n = circuit->log_n, log_l = s->log_l(), log_d = s->log_d();
-  const u64 n = 1ull << log_n;
   // the streamed plan evaluates the committed cosets [0, L) only (this rank's units of them): the LDE at factor L, whose
   // cosets are the first L of the factor-D domain with the same shifts, so the values and trees do not change.  The
   // quotient recomputes the other cosets from the borrowed natural-order columns.  The recompute plan keeps no coset: the
-  // tree is built one coset at a time, and s->tree.cols are the natural-order columns every reader rebuilds its cosets from.
-  if (s->recompute) {
-    BJ_TRY(oracle_build_by_coset(ctx, s->tree, {{d_sigmas, V}, {d_constants, C}, {d_lookup_tables, T}}, log_n, log_l,
-                                 circuit->merkle_tree_cap_size, circuit->tree_hasher, s->log_blocks));
-    return publish();
-  }
-  const uint32_t log_kept = s->streamed ? log_l : log_d;
-  s->col_len = (n << log_kept) / comm_world(ctx);
-  BJ_TRY(s->lde.alloc(ctx, (size_t)(V + C + T) * s->col_len));
-  BJ_TRY(lde_columns(ctx, d_sigmas, (uint64_t*)s->lde.p, log_n, log_kept, V));
-  if (C) BJ_TRY(lde_columns(ctx, d_constants, (uint64_t*)s->lde.p + (size_t)V * s->col_len, log_n, log_kept, C));
-  if (T) BJ_TRY(lde_columns(ctx, d_lookup_tables, (uint64_t*)s->lde.p + (size_t)(V + C) * s->col_len, log_n, log_kept, T));
-  for (uint32_t j = 0; j < V + C + T; j++) s->tree.cols.push_back(s->col(j));
-  BJ_TRY(oracle_build(ctx, s->tree, n << log_l, circuit->merkle_tree_cap_size, circuit->tree_hasher, circuit->fri_lde_factor));
-  if (s->compact) {
-    DevMem kept;
-    BJ_TRY(keep_first_cosets(ctx, s->tree.cols, n * circuit->quotient_degree, kept));
-    std::swap(s->lde.p, kept.p);
-    s->col_len = n * circuit->quotient_degree;
-  }
+  // tree is built one coset at a time, and s->cols.tree.cols are the natural-order columns every reader rebuilds its cosets from.
+  s->cols.init(s->plan, s->shape, {{d_sigmas, V}, {d_constants, C}, {d_lookup_tables, T}}, true);
+  BJ_TRY(s->cols.evaluate(ctx));
+  BJ_TRY(s->cols.build_tree(ctx, circuit->merkle_tree_cap_size, circuit->tree_hasher));
+  BJ_TRY(s->cols.keep_first_cosets(ctx));
   return publish();
 }
 
@@ -924,7 +1751,7 @@ void bj_setup_free(bj_setup* s) {
 
 int32_t bj_setup_get_cap(const bj_setup* s, uint64_t* h_cap) {
   if (!s || !h_cap) return BJ_ERR_INVALID_ARG;
-  memcpy(h_cap, s->tree.cap.data(), sizeof(uint64_t) * s->tree.cap.size());
+  memcpy(h_cap, s->cols.tree.cap.data(), sizeof(uint64_t) * s->cols.tree.cap.size());
   return BJ_OK;
 }
 
@@ -935,44 +1762,16 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: bad argument");
   if (setup->ctx != ctx) BJ_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, setup->ready, 0));
   const bj_circuit& c = setup->c;
-  const bool lk = c.lookup_width != 0;
-  if (lk && !d_multiplicities) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: the lookup argument needs the multiplicities column");
+  if (c.lookup_width && !d_multiplicities) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: the lookup argument needs the multiplicities column");
   *out = nullptr;
   std::unique_ptr<bj_proof> pf(new bj_proof());
   pf->c = c;
   pf->c.gates = nullptr;
-  const uint32_t V = c.num_variables, C = c.num_constants, Q = c.quotient_degree, L = c.fri_lde_factor, cap = c.merkle_tree_cap_size;
-  const uint32_t log_n = c.log_n, log_l = setup->log_l(), log_d = setup->log_d();
-  uint32_t log_q = 0;
-  while ((1u << log_q) < Q) log_q++;
-  const u64 n = 1ull << log_n, nQ = n << log_q;
-  // domain shard (multi-GPU): this context holds (L << split) / world units of every LDE column and its units of the first Q cosets
-  const uint32_t world = comm_world(ctx), rank = comm_rank(ctx);
-  const u64 nL = (n << log_l) / world;                                   // LOCAL length of the committed part of an LDE column
-  const u64 nD = (n << log_d) / world;                                   // LOCAL length (= stride) of an LDE column, D = max(L, Q)
-  const u64 nQl = ctx->shard.local_points(Q, (int)log_n);                 // LOCAL quotient points
-  const uint32_t split = ctx->shard.log_split;                            // 2^split row blocks per coset (split domain shard)
-  const u64 nb = n >> split;                                             // rows of one unit
-  const bool compact = setup->compact, streamed = setup->streamed, recompute = setup->recompute;
-  const uint32_t rb = setup->log_blocks;  // recompute plan on one GPU: 2^rb row blocks per coset in the trees and the quotient
-  const u64 Qn = n * Q;  // compact plan: elements of a setup / witness / stage-2 column kept on the device (cosets [0, Q))
-  const uint32_t log_kept = streamed ? log_l : log_d;  // streamed plan: those columns are evaluated on the cosets [0, L) only
-  const u64 nK = streamed ? nL : nD;      // stride of those columns on the resident and streamed plans
-  if (setup->col_len != (compact ? Qn : recompute ? 0 : nK))
-    BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: the setup was built with a different shard");
-  const uint32_t chunk = setup->chunk;  // compact and recompute plans: natural-order columns recomputed at a time
-  // the compact plan keeps cosets [0, Q) of the setup, witness and stage-2 columns, the recompute plan none: DEEP and the
-  // query answers rebuild the cosets [first_rebuilt, L) of them from the natural-order columns
-  const uint32_t first_rebuilt = compact ? Q : 0;
-  const u64 Fn = (u64)first_rebuilt * n;
+  if (!setup->cols.built_for(comm_world(ctx))) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: the setup was built with a different shard");
   {
     const uint64_t limit = ctx->memory_limit ? ctx->memory_limit : setup->limit;
-    if (setup->chosen_bytes() > limit) BJ_FAIL(ctx, BJ_ERR_OOM, plan_message("bj_prove", setup->plan, limit));
+    if (setup->chosen_bytes() > limit) BJ_FAIL(ctx, BJ_ERR_OOM, plan_message("bj_prove", setup->plan_bytes, limit));
   }
-  // Every DevMem below (and the FRI / query buffers of fri_driver.cu) is replayed by pool_peak in the same order: a new
-  // allocation here must be added there, or the plan no longer bounds the pool (tests/test_gpu_memory_budget.py pins the
-  // pool's high-water mark to the plan).
-  const uint32_t T = setup->n_tables, wdt = c.lookup_width, nsub = c.lookup_num_repetitions, voff = c.lookup_variables_offset;
   auto t_prev = std::chrono::steady_clock::now();
   auto mark = [&](int stage) -> int32_t {
     BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -981,813 +1780,21 @@ int32_t bj_prove(bj_ctx* ctx, const bj_setup* setup, const uint64_t* d_variables
     t_prev = now;
     return BJ_OK;
   };
-  struct TrGuard {
-    bj_transcript* t;
-    ~TrGuard() { bj_transcript_free(t); }
-  } trg{c.transcript == 1 ? bj_transcript_new_blake2s() : c.transcript == 2 ? bj_transcript_new_keccak256() : c.transcript == 3 ? bj_transcript_new_poseidon() : bj_transcript_new()};
-  bj_transcript* tr = trg.t;
-  auto challenge2 = [&]() {
-    gl::e2 r;
-    r.c0 = bj_transcript_get_challenge(tr);
-    r.c1 = bj_transcript_get_challenge(tr);
-    return r;
-  };
-  bj_transcript_witness_merkle_tree_cap(tr, (const uint64_t*)setup->tree.cap.data(), cap);  // prover.rs:211
-  // public inputs: read from the witness, committed to before anything else (prover.rs:264-266)
-  const uint32_t n_pi = c.n_public_inputs;
-  pf->public_inputs.resize(n_pi);
-  for (uint32_t i = 0; i < n_pi; i++)
-    BJ_CUDA(ctx, cudaMemcpyAsync(&pf->public_inputs[i], d_variables + ((size_t)setup->pi_cols[i] << c.log_n) + setup->pi_rows[i], sizeof(u64),
-                                 cudaMemcpyDeviceToHost, ctx->stream));
-  if (n_pi) BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  for (uint32_t i = 0; i < n_pi; i++) {
-    pf->public_inputs[i] = gl::canon(pf->public_inputs[i]);
-    const uint64_t v = pf->public_inputs[i];
-    bj_transcript_witness_field_elements(tr, &v, 1);
-  }
-
-  // ---- round 1: witness commitment ----
-  DevMem w_lde, m_lde;
-  ColumnGroups w_groups;  // compact plan
-  std::vector<const uint64_t*> w_cols(V);
-  const uint64_t* m_col = nullptr;
-  Oracle w_or;
-  if (recompute) {  // the tree one coset at a time; the columns stand for themselves in natural order from here on
-    BJ_TRY(oracle_build_by_coset(ctx, w_or, {{d_variables, V}, {d_multiplicities, lk ? 1u : 0u}}, log_n, log_l, cap, c.tree_hasher, rb));
-    for (uint32_t j = 0; j < V; j++) w_cols[j] = w_or.cols[j];
-    if (lk) m_col = w_or.cols[V];
-  } else if (compact) {
-    BJ_TRY(lde_grouped(ctx, w_groups, d_variables, V, log_n, log_d, w_cols.data()));
-    if (lk) BJ_TRY(lde_grouped(ctx, w_groups, d_multiplicities, 1, log_n, log_d, &m_col));
-  } else {
-    BJ_TRY(w_lde.alloc(ctx, (size_t)V * nK));
-    BJ_TRY(lde_columns(ctx, d_variables, (uint64_t*)w_lde.p, log_n, log_kept, V));
-    for (uint32_t j = 0; j < V; j++) w_cols[j] = (const uint64_t*)w_lde.p + (size_t)j * nK;
-    if (lk) {
-      BJ_TRY(m_lde.alloc(ctx, nK));
-      BJ_TRY(lde_columns(ctx, d_multiplicities, (uint64_t*)m_lde.p, log_n, log_kept, 1));
-      m_col = (const uint64_t*)m_lde.p;
-    }
-  }
-  if (!recompute) {
-    w_or.cols = w_cols;
-    if (lk) w_or.cols.push_back(m_col);  // variables | witness (none) | multiplicities
-    BJ_TRY(oracle_build(ctx, w_or, n << log_l, cap, c.tree_hasher, L));
-  }
-  pf->witness_cap = w_or.cap;
-  bj_transcript_witness_merkle_tree_cap(tr, (const uint64_t*)w_or.cap.data(), cap);
-  if (compact) {
-    BJ_TRY(keep_first_cosets_grouped(ctx, w_groups, w_or.cols, Qn));
-    for (uint32_t j = 0; j < V; j++) w_cols[j] = w_or.cols[j];
-    if (lk) m_col = w_or.cols[V];
-  }
+  Prover p(ctx, *setup, d_variables, d_multiplicities, *pf);
+  BJ_TRY(p.public_inputs());
+  BJ_TRY(p.round1());
   BJ_TRY(mark(0));
-
-  // ---- round 2: copy-permutation grand product, partial products, lookup polynomials ----
-  const gl::e2 beta = challenge2(), gamma = challenge2();
-  gl::e2 lookup_beta{0, 0}, lookup_gamma{0, 0};
-  if (lk) {
-    lookup_beta = challenge2();  // prover.rs:402-406
-    lookup_gamma = challenge2();
-  }
-  const uint32_t n_chunks = (V + Q - 1) / Q, n_partial = n_chunks - 1;
-  const uint32_t n_s2 = 2 + 2 * n_partial + (lk ? 2 * (nsub + 1) : 0);  // z | partials | A_i | B   (c0, c1 each)
-  DevMem st2, s2_lde;
-  BJ_TRY(st2.alloc(ctx, (size_t)n_s2 * n));
-  {
-    std::vector<const uint64_t*> vp(V), sp(V);
-    for (uint32_t j = 0; j < V; j++) {
-      vp[j] = d_variables + (size_t)j * n;
-      sp[j] = setup->sigmas + (size_t)j * n;
-    }
-    std::vector<uint64_t> nr(V);
-    BJ_TRY(bj_non_residues_for_copy_permutation(n, V, nr.data()));
-    const uint64_t b[2] = {beta.c0, beta.c1}, g[2] = {gamma.c0, gamma.c1};
-    if (world > 1 && n >= (u64)world * 16)  // rows split over the ranks, one all-gather (stage2.cu)
-      BJ_TRY(copy_permutation_stage2_sharded(ctx, vp.data(), sp.data(), V, nr.data(), beta, gamma, log_n, Q, st2.p));
-    else
-      BJ_TRY(bj_copy_permutation_stage2(ctx, vp.data(), sp.data(), V, nr.data(), b, g, log_n, Q, (uint64_t*)st2.p, (uint64_t*)st2.p + n,
-                                        (uint64_t*)st2.p + 2 * n));
-    if (lk) {
-      std::vector<const uint64_t*> lc(wdt * nsub), tc(T);
-      for (uint32_t i = 0; i < wdt * nsub; i++) lc[i] = d_variables + (size_t)(voff + i) * n;
-      for (uint32_t j = 0; j < T; j++) tc[j] = setup->tables + (size_t)j * n;
-      const uint64_t lb[2] = {lookup_beta.c0, lookup_beta.c1}, lg[2] = {lookup_gamma.c0, lookup_gamma.c1};
-      BJ_TRY(bj_lookup_polys_specialized(ctx, lc.data(), nsub, wdt, setup->constants + (size_t)c.lookup_table_id_column * n, tc.data(), T,
-                                         d_multiplicities, lb, lg, log_n, (uint64_t*)st2.p + (size_t)(2 + 2 * n_partial) * n));
-    }
-  }
-  ColumnGroups s2_groups;  // compact plan
-  std::vector<const uint64_t*> s2_cols(n_s2);
-  Oracle s2_or;
-  if (recompute) {
-    BJ_TRY(oracle_build_by_coset(ctx, s2_or, {{(const uint64_t*)st2.p, n_s2}}, log_n, log_l, cap, c.tree_hasher, rb));
-    s2_cols = s2_or.cols;
-  } else if (compact) {
-    BJ_TRY(lde_grouped(ctx, s2_groups, (const uint64_t*)st2.p, n_s2, log_n, log_d, s2_cols.data()));
-  } else {
-    BJ_TRY(s2_lde.alloc(ctx, (size_t)n_s2 * nK));
-    BJ_TRY(lde_columns(ctx, (const uint64_t*)st2.p, (uint64_t*)s2_lde.p, log_n, log_kept, n_s2));
-    for (uint32_t j = 0; j < n_s2; j++) s2_cols[j] = (const uint64_t*)s2_lde.p + (size_t)j * nK;
-  }
-  // a row block of a split shard does not hold z(omega x) (another block of the coset does).  On a unit with shift sigma,
-  // z(omega x) is the LDE of z on the shift sigma * omega in the same row order: two more columns (c0, c1 of z).  The
-  // streamed and recompute plans evaluate them one unit at a time with the quotient's other columns.
-  DevMem z_next;
-  if (split && !streamed && !recompute && ctx->shard.local_units(Q)) {
-    BJ_TRY(z_next.alloc(ctx, 2 * nD));
-    BJ_TRY(bj_lde_next_row(ctx, (const uint64_t*)st2.p, n, (uint64_t*)z_next.p, log_n, log_d, 2, 0));
-  }
-  // the compact plan recomputes cosets [Q, L) of stage 2 from it, the streamed [L, Q), the recompute plan every coset
-  if (!compact && !streamed && !recompute) st2.release();
-  if (!recompute) {
-    s2_or.cols = s2_cols;
-    BJ_TRY(oracle_build(ctx, s2_or, n << log_l, cap, c.tree_hasher, L));
-  }
-  pf->stage2_cap = s2_or.cap;
-  bj_transcript_witness_merkle_tree_cap(tr, (const uint64_t*)s2_or.cap.data(), cap);
-  if (compact) {
-    BJ_TRY(keep_first_cosets_grouped(ctx, s2_groups, s2_or.cols, Qn));
-    s2_cols = s2_or.cols;
-  }
-  const uint32_t a_off = 2 + 2 * n_partial;
+  BJ_TRY(p.round2());
   BJ_TRY(mark(1));
-
-  // ---- round 3: quotient ----
-  const gl::e2 alpha = challenge2();
-  uint32_t n_gate_terms = 0;
-  for (const auto& g : setup->gates) n_gate_terms += g.n_writes * g.num_repetitions;
-  const uint32_t n_lk_terms = lk ? nsub + 1 : 0;  // lookup terms come first (prover.rs:608-625)
-  const uint32_t total_terms = n_lk_terms + n_gate_terms + 1 + 1 + n_partial;
-  std::vector<uint64_t> powers(2 * (size_t)total_terms);
-  {
-    gl::e2 cur{1, 0};
-    for (uint32_t i = 0; i < total_terms; i++) {
-      powers[2 * i] = cur.c0;
-      powers[2 * i + 1] = cur.c1;
-      cur = gl::e2_mul(cur, alpha);
-    }
-  }
-  std::vector<const uint64_t*> const_cols(C), sigma_cols(V), table_cols(T);
-  // the setup tree's columns: the kept LDE columns, or on the recompute plan the natural-order ones
-  for (uint32_t j = 0; j < V; j++) sigma_cols[j] = setup->tree.cols[j];
-  for (uint32_t j = 0; j < C; j++) const_cols[j] = setup->tree.cols[V + j];
-  for (uint32_t j = 0; j < T; j++) table_cols[j] = setup->tree.cols[V + C + j];
-  DevMem qq, qloc;  // qq: [2][nQ] global (c0 then c1); qloc: this rank's cosets among the first Q
-  BJ_TRY(qq.alloc(ctx, 2 * nQ));
-  uint64_t* q0 = (uint64_t*)qq.p;
-  uint64_t* q1 = q0 + nQ;
-  uint64_t* const gq0 = q0;
-  uint64_t* const gq1 = q1;
-  if (world > 1) {
-    BJ_TRY(qloc.alloc(ctx, 2 * std::max<u64>(nQl, 1)));
-    q0 = (uint64_t*)qloc.p;
-    q1 = q0 + nQl;
-    BJ_CUDA(ctx, cudaMemsetAsync(qloc.p, 0, sizeof(u64) * 2 * std::max<u64>(nQl, 1), ctx->stream));
-  } else {
-    BJ_CUDA(ctx, cudaMemsetAsync(qq.p, 0, sizeof(u64) * 2 * nQ, ctx->stream));
-  }
-  // the quotient's terms and the division by the vanishing polynomial on the n_points points the context's shard reads, from
-  // the LDE columns of what the quotient reads (variables, multiplicities, sigmas, constants, tables, stage 2)
-  struct QuotientCols {
-    std::vector<const uint64_t*> w, sigma, consts, tables, s2;
-    const uint64_t* m;
-    const uint64_t *z_next0, *z_next1;  // split shard: z(omega x) on the same points
-  };
-  auto quotient_terms = [&](const QuotientCols& k, u64 n_points, uint64_t* o0, uint64_t* o1) -> int32_t {
-    if (lk) {
-      std::vector<const uint64_t*> ll(wdt * nsub), al(2 * nsub);
-      for (uint32_t i = 0; i < wdt * nsub; i++) ll[i] = k.w[voff + i];
-      for (uint32_t i = 0; i < 2 * nsub; i++) al[i] = k.s2[a_off + i];
-      const uint64_t lb[2] = {lookup_beta.c0, lookup_beta.c1}, lg[2] = {lookup_gamma.c0, lookup_gamma.c1};
-      BJ_TRY(bj_quotient_lookup_specialized(ctx, ll.data(), nsub, wdt, k.consts[c.lookup_table_id_column], k.tables.data(), T,
-                                            k.m, al.data(), k.s2[a_off + 2 * nsub], k.s2[a_off + 2 * nsub + 1], lb, lg,
-                                            powers.data(), n_points, o0, o1));
-    }
-    if (n_gate_terms)
-      BJ_TRY(bj_quotient_gates_general_purpose(ctx, setup->gates.data(), (uint32_t)setup->gates.size(), k.w.data(), V, nullptr, 0,
-                                               k.consts.data(), C, powers.data() + 2 * (size_t)n_lk_terms, n_gate_terms, n_points, o0, o1));
-    {
-      std::vector<uint64_t> nr(V);
-      BJ_TRY(bj_non_residues_for_copy_permutation(n, V, nr.data()));
-      const uint64_t b[2] = {beta.c0, beta.c1}, g[2] = {gamma.c0, gamma.c1};
-      if (ctx->shard.log_split)  // a row block (split shard, or a recompute unit under its window) does not hold z(omega x)
-        BJ_TRY(bj_quotient_copy_permutation_with_z_next(ctx, k.w.data(), k.sigma.data(), V, nr.data(), k.s2[0], k.s2[1], k.z_next0,
-                                                        k.z_next1, n_partial ? k.s2.data() + 2 : nullptr, b, g,
-                                                        powers.data() + 2 * (size_t)(n_lk_terms + n_gate_terms), log_n, log_d, log_q, Q, o0, o1));
-      else
-        BJ_TRY(bj_quotient_copy_permutation(ctx, k.w.data(), k.sigma.data(), V, nr.data(), k.s2[0], k.s2[1],
-                                            n_partial ? k.s2.data() + 2 : nullptr, b, g, powers.data() + 2 * (size_t)(n_lk_terms + n_gate_terms),
-                                            log_n, log_d, log_q, Q, o0, o1));
-    }
-    return bj_quotient_divide_by_vanishing(ctx, o0, o1, log_n, log_q);
-  };
-  if (!streamed && !recompute) {
-    const uint64_t* zn = (const uint64_t*)z_next.p;
-    if (nQl) BJ_TRY(quotient_terms({w_cols, sigma_cols, const_cols, table_cols, s2_cols, m_col, zn, zn ? zn + nD : nullptr}, nQl, q0, q1));
-  } else {
-    // one local quotient unit k at a time (global unit u: coset u on one GPU or a coset shard, a row block of ub rows of
-    // coset u / B on a split shard or on one GPU with 2^rb row blocks per coset), under the window of unit u among the units
-    // of the factor-D domain.  On the streamed plan the units of the committed cosets [0, L) come from the kept columns
-    // (their first L * B / world local units); the others, and every unit on the recompute plan, are evaluated into one
-    // unit-sized scratch from the natural-order columns; on a row block the unit's z(omega x) columns go to the scratch too.
-    // The unit's quotient values land in its slot [k ub, (k + 1) ub) of the local quotient cosets.
-    CosetShard shard = ctx->shard;
-    shard.log_split += rb;  // one GPU: every one of the Q * 2^rb units is local, global unit k = k
-    const uint32_t usplit = shard.log_split;
-    const u64 ub = n >> usplit;
-    const u64 q_units = shard.local_units(Q), kept_units = recompute ? 0 : shard.local_units(L);
-    DevMem ev;
-    BJ_TRY(ev.alloc(ctx, (size_t)(2 * V + C + T + (lk ? 1 : 0) + n_s2 + (usplit ? 2 : 0)) * ub));
-    for (u64 k = 0; k < q_units; k++) {
-      ShardWindow window(ctx, log_d + usplit, (u32)shard.global_unit(k), usplit);
-      QuotientCols qc;
-      uint64_t* e = (uint64_t*)ev.p;
-      // columns `kept` moved to unit k, or `cnt` natural columns of `nat` evaluated on unit u into the next slots of ev
-      // (bj_lde under the window: the same coset transform, or fold + row-block transform, as the resident plan's LDE)
-      auto unit_k = [&](const std::vector<const uint64_t*>& kept_cols, const uint64_t* nat, uint32_t cnt, std::vector<const uint64_t*>& out) -> int32_t {
-        out.resize(cnt);
-        if (k < kept_units) {
-          for (uint32_t i = 0; i < cnt; i++) out[i] = kept_cols[i] + (size_t)k * ub;
-          return BJ_OK;
-        }
-        if (cnt) BJ_TRY(bj_lde(ctx, nat, n, e, log_n, log_d, cnt, 0));
-        for (uint32_t i = 0; i < cnt; i++) out[i] = e + (size_t)i * ub;
-        e += (size_t)cnt * ub;
-        return BJ_OK;
-      };
-      BJ_TRY(unit_k(w_cols, d_variables, V, qc.w));
-      BJ_TRY(unit_k(sigma_cols, setup->sigmas, V, qc.sigma));
-      BJ_TRY(unit_k(const_cols, setup->constants, C, qc.consts));
-      BJ_TRY(unit_k(table_cols, setup->tables, T, qc.tables));
-      BJ_TRY(unit_k(s2_cols, (const uint64_t*)st2.p, n_s2, qc.s2));
-      std::vector<const uint64_t*> mj;
-      if (lk) BJ_TRY(unit_k({m_col}, d_multiplicities, 1, mj));
-      qc.m = lk ? mj[0] : nullptr;
-      qc.z_next0 = qc.z_next1 = nullptr;
-      if (usplit) {
-        BJ_TRY(bj_lde_next_row(ctx, (const uint64_t*)st2.p, n, e, log_n, log_d, 2, 0));
-        qc.z_next0 = e;
-        qc.z_next1 = e + ub;
-      }
-      BJ_TRY(quotient_terms(qc, ub, q0 + (size_t)k * ub, q1 + (size_t)k * ub));
-    }
-  }
-  z_next.release();
-  if (world > 1) {
-    // the one bulk exchange: the quotient cosets recombine (they are interpolated together at size n * Q).  Every rank sends
-    // `per` = ceil(Q * B / world) unit slots of nb = n / B rows (c0 | c1 per slot; ranks beyond the Q * B units send
-    // padding), one all-gather, then the slots are scattered to their global unit positions.
-    const u64 q_units = (u64)Q << split;
-    const u64 per = std::max<u64>(1, q_units / world);
-    DevMem snd, rcv;
-    BJ_TRY(snd.alloc(ctx, per * 2 * nb));
-    BJ_TRY(rcv.alloc(ctx, (u64)world * per * 2 * nb));
-    BJ_CUDA(ctx, cudaMemsetAsync(snd.p, 0, sizeof(u64) * per * 2 * nb, ctx->stream));
-    const u64 q_loc = ctx->shard.local_units(Q);
-    for (u64 k = 0; k < q_loc; k++) {
-      BJ_CUDA(ctx, cudaMemcpyAsync(snd.p + (2 * k) * nb, q0 + k * nb, sizeof(u64) * nb, cudaMemcpyDeviceToDevice, ctx->stream));
-      BJ_CUDA(ctx, cudaMemcpyAsync(snd.p + (2 * k + 1) * nb, q1 + k * nb, sizeof(u64) * nb, cudaMemcpyDeviceToDevice, ctx->stream));
-    }
-    BJ_TRY(comm_all_gather(ctx->comm, snd.p, rcv.p, per * 2 * nb));
-    for (uint32_t r = 0; r < world; r++)
-      for (u64 k = 0; k < per; k++) {
-        const u64 u = ctx->shard.unit_of(r, k);
-        if (u >= q_units) continue;
-        const u64* part = rcv.p + ((u64)r * per + k) * 2 * nb;
-        BJ_CUDA(ctx, cudaMemcpyAsync(gq0 + u * nb, part, sizeof(u64) * nb, cudaMemcpyDeviceToDevice, ctx->stream));
-        BJ_CUDA(ctx, cudaMemcpyAsync(gq1 + u * nb, part + nb, sizeof(u64) * nb, cudaMemcpyDeviceToDevice, ctx->stream));
-      }
-    q0 = gq0;
-    q1 = gq1;
-    qloc.release();
-  }
-  // cosets -> natural order, one interpolation of size n*Q on the coset 7, Q chunks of n coefficients (prover.rs:1399-1467)
-  BJ_TRY(bj_bitreverse(ctx, q0, log_n + log_q, 2, nQ));
-  BJ_TRY(bj_intt_natural_to_natural(ctx, q0, log_n + log_q, 2, nQ, gl::MULT_GEN));
-  {
-    // the reference's satisfiability guard: the top coefficient must vanish (prover.rs:1425-1438)
-    uint64_t top[2];
-    BJ_CUDA(ctx, cudaMemcpyAsync(&top[0], q0 + nQ - 1, sizeof(u64), cudaMemcpyDeviceToHost, ctx->stream));
-    BJ_CUDA(ctx, cudaMemcpyAsync(&top[1], q1 + nQ - 1, sizeof(u64), cudaMemcpyDeviceToHost, ctx->stream));
-    BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (top[0] || top[1]) BJ_FAIL(ctx, BJ_ERR_INVALID_ARG, "bj_prove: unsatisfied circuit (quotient is not a polynomial of degree < n * quotient_degree)");
-  }
-  DevMem chunks, qt_lde;  // chunk j: c0 then c1
-  BJ_TRY(chunks.alloc(ctx, 2 * nQ));
-  for (uint32_t j = 0; j < Q; j++) {
-    BJ_CUDA(ctx, cudaMemcpyAsync(chunks.p + (size_t)(2 * j) * n, q0 + (size_t)j * n, sizeof(u64) * n, cudaMemcpyDeviceToDevice, ctx->stream));
-    BJ_CUDA(ctx, cudaMemcpyAsync(chunks.p + (size_t)(2 * j + 1) * n, q1 + (size_t)j * n, sizeof(u64) * n, cudaMemcpyDeviceToDevice, ctx->stream));
-  }
-  qq.release();
-  BJ_TRY(qt_lde.alloc(ctx, (size_t)(2 * Q) * nL));
-  BJ_TRY(bj_lde(ctx, (const uint64_t*)chunks.p, n, (uint64_t*)qt_lde.p, log_n, log_l, 2 * Q, 1));
-  chunks.release();
-  std::vector<const uint64_t*> qt_cols(2 * Q);
-  for (uint32_t j = 0; j < 2 * Q; j++) qt_cols[j] = (const uint64_t*)qt_lde.p + (size_t)j * nL;
-  Oracle qt_or;
-  qt_or.cols = qt_cols;
-  BJ_TRY(oracle_build(ctx, qt_or, n << log_l, cap, c.tree_hasher, L));
-  pf->quotient_cap = qt_or.cap;
-  bj_transcript_witness_merkle_tree_cap(tr, (const uint64_t*)qt_or.cap.data(), cap);
+  BJ_TRY(p.quotient());
   BJ_TRY(mark(2));
-
-  // ---- round 4: openings.  Order (prover.rs:1549-1683): variables, witness, constants, sigmas, z, partial products,
-  //      multiplicities, lookup A, lookup B, lookup tables, quotient chunks.
-  const gl::e2 z = challenge2();
-  const gl::e2 z_omega = gl::e2_mul_base(z, gl::omega(log_n));
-  struct Src {
-    const uint64_t* c0;
-    const uint64_t* c1;  // nullptr: base-field polynomial
-  };
-  std::vector<Src> sources;
-  for (uint32_t j = 0; j < V; j++) sources.push_back({w_cols[j], nullptr});
-  for (uint32_t j = 0; j < C; j++) sources.push_back({const_cols[j], nullptr});
-  for (uint32_t j = 0; j < V; j++) sources.push_back({sigma_cols[j], nullptr});
-  for (uint32_t i = 0; i < 1 + n_partial; i++) sources.push_back({s2_cols[2 * i], s2_cols[2 * i + 1]});
-  std::vector<Src> zero_sources;
-  if (lk) {
-    sources.push_back({m_col, nullptr});
-    for (uint32_t i = 0; i < nsub + 1; i++) {
-      sources.push_back({s2_cols[a_off + 2 * i], s2_cols[a_off + 2 * i + 1]});
-      zero_sources.push_back({s2_cols[a_off + 2 * i], s2_cols[a_off + 2 * i + 1]});
-    }
-    for (uint32_t j = 0; j < T; j++) sources.push_back({table_cols[j], nullptr});
-  }
-  for (uint32_t i = 0; i < Q; i++) sources.push_back({qt_cols[2 * i], qt_cols[2 * i + 1]});
-  // compact and recompute plans: the natural-order columns behind the setup, witness and stage-2 oracles, in the order of
-  // the oracles' columns (so a row of them is the three oracles' leaves side by side), and the kept LDE column of each (on
-  // the recompute plan the oracles' columns are the natural ones themselves)
-  std::vector<const uint64_t*> nat;
-  std::unordered_map<const uint64_t*, uint32_t> nat_of;  // kept LDE column -> its index in nat
-  std::vector<char> pair_start;                          // nat[i], nat[i + 1] are the c0, c1 of one Fp2 polynomial
-  const uint32_t S = V + C + T;
-  if (compact || recompute) {
-    for (uint32_t j = 0; j < V; j++) nat.push_back(setup->sigmas + (size_t)j * n);
-    for (uint32_t j = 0; j < C; j++) nat.push_back(setup->constants + (size_t)j * n);
-    for (uint32_t j = 0; j < T; j++) nat.push_back(setup->tables + (size_t)j * n);
-    for (uint32_t j = 0; j < V; j++) nat.push_back(d_variables + (size_t)j * n);
-    if (lk) nat.push_back(d_multiplicities);
-    for (uint32_t j = 0; j < n_s2; j++) nat.push_back((const uint64_t*)st2.p + (size_t)j * n);
-    std::vector<const uint64_t*> kept(setup->tree.cols);
-    kept.insert(kept.end(), w_or.cols.begin(), w_or.cols.end());
-    kept.insert(kept.end(), s2_or.cols.begin(), s2_or.cols.end());
-    for (uint32_t i = 0; i < kept.size(); i++) nat_of[kept[i]] = i;
-    pair_start.assign(nat.size(), 0);
-    for (uint32_t j = 0; j < n_s2; j += 2) pair_start[S + w_or.cols.size() + j] = 1;
-  }
-  // chunks of `chunk` natural columns among nat[lo, hi) (an Fp2 pair never split): monomials by one iNTT, then body(c0, cnt,
-  // monomials, scratch for one unit of the chunk: a coset, or nb rows of one on a split shard, stride nb)
-  auto for_chunks = [&](uint32_t lo, uint32_t hi, const std::function<int32_t(uint32_t, uint32_t, const uint64_t*, uint64_t*)>& body) -> int32_t {
-    DevMem mono, ev;
-    BJ_TRY(mono.alloc(ctx, (size_t)chunk * n));
-    BJ_TRY(ev.alloc(ctx, (size_t)chunk * nb));
-    for (uint32_t c0 = lo; c0 < hi;) {
-      uint32_t cnt = std::min<uint32_t>(chunk, hi - c0);
-      if (c0 + cnt < hi && pair_start[c0 + cnt - 1]) cnt--;
-      for (uint32_t i = 0; i < cnt; i++)
-        BJ_CUDA(ctx, cudaMemcpyAsync(mono.p + (size_t)i * n, nat[c0 + i], sizeof(u64) * n, cudaMemcpyDeviceToDevice, ctx->stream));
-      BJ_TRY(bj_intt_natural_to_natural(ctx, (uint64_t*)mono.p, log_n, cnt, n, 1));
-      BJ_TRY(body(c0, cnt, (const uint64_t*)mono.p, (uint64_t*)ev.p));
-      c0 += cnt;
-    }
-    return BJ_OK;
-  };
-  // recompute plan: the barycentric sums of the natural columns among flat from local slot 0 (coset 0 on one GPU, this rank's
-  // coset or row block on a sharded context), rebuilt a chunk at a time (only the chunks that hold one of them), those of the
-  // quotient oracle's columns directly
-  auto open_rebuilt = [&](const std::vector<const uint64_t*>& flat, const uint64_t a[2], uint64_t* ev) -> int32_t {
-    auto evaluate = [&](const std::vector<const uint64_t*>& cols, const std::vector<size_t>& at) -> int32_t {
-      if (cols.empty()) return BJ_OK;
-      std::vector<uint64_t> got(2 * cols.size());
-      BJ_TRY(bj_barycentric_evaluate(ctx, cols.data(), (uint32_t)cols.size(), log_n, a, got.data()));
-      for (size_t k = 0; k < at.size(); k++) {
-        ev[2 * at[k]] = got[2 * k];
-        ev[2 * at[k] + 1] = got[2 * k + 1];
-      }
-      return BJ_OK;
-    };
-    std::vector<const uint64_t*> direct;
-    std::vector<size_t> direct_at;
-    uint32_t lo = (uint32_t)nat.size(), hi = 0;
-    for (size_t i = 0; i < flat.size(); i++) {
-      const auto it = nat_of.find(flat[i]);
-      if (it == nat_of.end()) {
-        direct.push_back(flat[i]);
-        direct_at.push_back(i);
-      } else {
-        lo = std::min(lo, it->second);
-        hi = std::max(hi, it->second + 1);
-      }
-    }
-    BJ_TRY(evaluate(direct, direct_at));
-    return for_chunks(lo, hi, [&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* on_coset) -> int32_t {
-      BJ_TRY(lde_unit(ctx, mono, on_coset, log_n, log_l, cnt, 0, 1));
-      std::vector<const uint64_t*> cols;
-      std::vector<size_t> at;
-      for (size_t i = 0; i < flat.size(); i++) {
-        const auto it = nat_of.find(flat[i]);
-        if (it == nat_of.end() || it->second < c0 || it->second >= c0 + cnt) continue;
-        cols.push_back(on_coset + (size_t)(it->second - c0) * nb);
-        at.push_back(i);
-      }
-      return evaluate(cols, at);
-    });
-  };
-  auto open_at = [&](const std::vector<Src>& srcs, gl::e2 at, std::vector<gl::e2>& vals) -> int32_t {
-    std::vector<const uint64_t*> flat;
-    for (const auto& s : srcs) {
-      flat.push_back(s.c0);
-      if (s.c1) flat.push_back(s.c1);
-    }
-    vals.clear();
-    if (flat.empty()) return BJ_OK;
-    std::vector<uint64_t> ev(2 * flat.size());
-    const uint64_t a[2] = {at.c0, at.c1};
-    if (world == 1) {
-      if (recompute) BJ_TRY(open_rebuilt(flat, a, ev.data()));
-      else BJ_TRY(bj_barycentric_evaluate(ctx, flat.data(), (uint32_t)flat.size(), log_n, a, ev.data()));
-    } else {
-      // the columns are split over the coset groups: ranks [g B, (g + 1) B) hold the B row blocks of coset g (B = 1: one rank,
-      // its whole coset) and open column block g from it, each rank its block's contribution (on the recompute plan from its
-      // rebuilt local slot 0).  The contributions are gathered and the B of a group summed.
-      const uint32_t groups = world >> split, g = rank >> split;
-      const size_t per = (flat.size() + groups - 1) / groups, first = std::min(flat.size(), (size_t)g * per);
-      const size_t cnt = std::min(per, flat.size() - first);
-      std::vector<uint64_t> mine(2 * per, 0), all(2 * per * world);
-      if (cnt && recompute)
-        BJ_TRY(open_rebuilt(std::vector<const uint64_t*>(flat.begin() + first, flat.begin() + first + cnt), a, mine.data()));
-      else if (cnt)
-        BJ_TRY(bj_barycentric_evaluate(ctx, flat.data() + first, (uint32_t)cnt, log_n, a, mine.data()));
-      BJ_TRY(comm_all_gather_host(ctx->comm, (const u64*)mine.data(), (u64*)all.data(), 2 * per));
-      for (uint32_t gg = 0; gg < groups; gg++)
-        for (size_t e = 0; e < 2 * per && gg * 2 * per + e < ev.size(); e++) {
-          u64 v = 0;
-          for (uint32_t p = 0; p < (1u << split); p++) v = gl::canon(gl::add(v, all[(((size_t)gg << split) + p) * 2 * per + e]));
-          ev[gg * 2 * per + e] = v;   // group blocks are contiguous: [g][per] == flat order
-        }
-    }
-    size_t k = 0;
-    for (const auto& s : srcs) {
-      if (s.c1) {  // f0 + u f1 at an Fp2 point (u^2 = 7)
-        const gl::e2 a0{ev[2 * k], ev[2 * k + 1]}, b0{ev[2 * k + 2], ev[2 * k + 3]};
-        vals.push_back({gl::canon(gl::add(a0.c0, gl::mul7(b0.c1))), gl::canon(gl::add(a0.c1, b0.c0))});
-        k += 2;
-      } else {
-        vals.push_back({ev[2 * k], ev[2 * k + 1]});
-        k += 1;
-      }
-    }
-    return BJ_OK;
-  };
-  std::vector<Src> z_omega_sources{{s2_cols[0], s2_cols[1]}};
-  BJ_TRY(open_at(sources, z, pf->values_at_z));
-  BJ_TRY(open_at(z_omega_sources, z_omega, pf->values_at_z_omega));
-  BJ_TRY(open_at(zero_sources, gl::e2{0, 0}, pf->values_at_0));
-  for (const auto* vs : {&pf->values_at_z, &pf->values_at_z_omega, &pf->values_at_0})
-    for (const auto& v : *vs) {
-      const uint64_t e[2] = {v.c0, v.c1};
-      bj_transcript_witness_field_elements(tr, e, 2);
-    }
+  BJ_TRY(p.openings());
   BJ_TRY(mark(3));
-
-  // ---- round 5: DEEP combination + FRI ----
-  // public inputs grouped by opening point w^row in order of first appearance (prover.rs:1805-1821)
-  struct PiGroup {
-    u64 at;
-    std::vector<Src> srcs;
-    std::vector<gl::e2> vals;
-  };
-  std::vector<PiGroup> pi_groups;
-  for (uint32_t i = 0; i < n_pi; i++) {
-    const u64 at = gl::pow(gl::omega(log_n), setup->pi_rows[i]);
-    PiGroup* g = nullptr;
-    for (auto& e : pi_groups)
-      if (e.at == at) g = &e;
-    if (!g) {
-      pi_groups.push_back({at, {}, {}});
-      g = &pi_groups.back();
-    }
-    g->srcs.push_back({w_cols[setup->pi_cols[i]], nullptr});
-    g->vals.push_back({pf->public_inputs[i], 0});
-  }
-  const gl::e2 ch0 = challenge2();
-  const size_t n_ch = pf->values_at_z.size() + 1 + pf->values_at_0.size() + n_pi;
-  std::vector<uint64_t> ch(2 * n_ch);
-  {
-    gl::e2 cur{1, 0};
-    for (size_t i = 0; i < n_ch; i++) {
-      ch[2 * i] = cur.c0;
-      ch[2 * i + 1] = cur.c1;
-      cur = gl::e2_mul(cur, ch0);
-    }
-  }
-  DevMem deep;
-  BJ_TRY(deep.alloc(ctx, 2 * nL));
-  BJ_CUDA(ctx, cudaMemsetAsync(deep.p, 0, sizeof(u64) * 2 * nL, ctx->stream));
-  struct DeepGroup {
-    const std::vector<Src>* srcs;
-    const std::vector<gl::e2>* vals;
-    gl::e2 at;
-    const uint64_t* chs;
-  };
-  std::vector<DeepGroup> deep_groups;
-  // sources i of a group with keep(i) on the local points [first, first + count), column pointers moved by at_col.  One GPU:
-  // any run of points.  Sharded (recompute plan): the whole local domain, or local unit k (first = k nb, count = nb) under
-  // its window, whose points the kernel then places at their global indices.
-  auto deep_range = [&](const DeepGroup& g, const std::function<bool(size_t)>& keep, const std::function<const uint64_t*(const uint64_t*)>& at_col,
-                        u64 first, u64 count) -> int32_t {
-    std::vector<const uint64_t*> p0, p1;
-    std::vector<uint64_t> v, ch;
-    for (size_t i = 0; i < g.srcs->size(); i++) {
-      if (!keep(i)) continue;
-      const Src& sr = (*g.srcs)[i];
-      p0.push_back(at_col(sr.c0));
-      p1.push_back(sr.c1 ? at_col(sr.c1) : nullptr);
-      v.push_back((*g.vals)[i].c0);
-      v.push_back((*g.vals)[i].c1);
-      ch.push_back(g.chs[2 * i]);
-      ch.push_back(g.chs[2 * i + 1]);
-    }
-    if (p0.empty()) return BJ_OK;
-    const uint64_t a[2] = {g.at.c0, g.at.c1};
-    uint64_t *acc0 = (uint64_t*)deep.p + first, *acc1 = (uint64_t*)deep.p + nL + first;
-    if (world == 1)
-      return bj_deep_quotient_range(ctx, p0.data(), p1.data(), (uint32_t)p0.size(), v.data(), ch.data(), a, log_n + log_l, first, count, acc0, acc1);
-    if (count == nL)
-      return bj_deep_quotient_group(ctx, p0.data(), p1.data(), (uint32_t)p0.size(), v.data(), ch.data(), a, log_n + log_l, acc0, acc1);
-    ShardWindow window(ctx, log_l + split, (u32)ctx->shard.global_unit(first / nb), split);
-    return bj_deep_quotient_group(ctx, p0.data(), p1.data(), (uint32_t)p0.size(), v.data(), ch.data(), a, log_n + log_l, acc0, acc1);
-  };
-  auto deep_group = [&](const std::vector<Src>& srcs, const std::vector<gl::e2>& vals, gl::e2 at, const uint64_t* chs) -> int32_t {
-    if (srcs.empty()) return BJ_OK;
-    if (compact || recompute) {
-      // cosets [0, first_rebuilt) from the kept columns; the quotient oracle's columns hold all L cosets; the rest is
-      // recomputed below
-      const DeepGroup g{&srcs, &vals, at, chs};
-      deep_groups.push_back(g);
-      if (Fn) BJ_TRY(deep_range(g, [](size_t) { return true; }, [](const uint64_t* p) { return p; }, 0, Fn));
-      return deep_range(g, [&](size_t i) { return !nat_of.count(srcs[i].c0); }, [&](const uint64_t* p) { return p + Fn; }, Fn, nL - Fn);
-    }
-    std::vector<const uint64_t*> p0(srcs.size()), p1(srcs.size());
-    std::vector<uint64_t> v(2 * srcs.size());
-    for (size_t i = 0; i < srcs.size(); i++) {
-      p0[i] = srcs[i].c0;
-      p1[i] = srcs[i].c1;
-      v[2 * i] = vals[i].c0;
-      v[2 * i + 1] = vals[i].c1;
-    }
-    const uint64_t a[2] = {at.c0, at.c1};
-    return bj_deep_quotient_group(ctx, p0.data(), p1.data(), (uint32_t)srcs.size(), v.data(), chs, a, log_n + log_l /* global */,
-                                  (uint64_t*)deep.p, (uint64_t*)deep.p + nL);
-  };
-  BJ_TRY(deep_group(sources, pf->values_at_z, z, ch.data()));
-  BJ_TRY(deep_group(z_omega_sources, pf->values_at_z_omega, z_omega, ch.data() + 2 * sources.size()));
-  BJ_TRY(deep_group(zero_sources, pf->values_at_0, gl::e2{0, 0}, ch.data() + 2 * (sources.size() + 1)));
-  {
-    size_t off = sources.size() + 1 + zero_sources.size();
-    for (const auto& g : pi_groups) {  // prover.rs:2010-2041
-      BJ_TRY(deep_group(g.srcs, g.vals, gl::e2{g.at, 0}, ch.data() + 2 * off));
-      off += g.srcs.size();
-    }
-  }
-  // local units of the committed cosets [0, L): the cosets themselves on one GPU, this rank's units on a sharded context
-  const u64 units_l = ctx->shard.local_units(L);
-  if (compact || recompute)  // units [first_rebuilt, units_l): every chunk of natural columns evaluated on one unit at a time, its DEEP terms added
-    BJ_TRY(for_chunks(0, (uint32_t)nat.size(), [&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* ev) -> int32_t {
-      auto in_chunk = [&](const uint64_t* p) {
-        const auto it = nat_of.find(p);
-        return it != nat_of.end() && it->second >= c0 && it->second < c0 + cnt;
-      };
-      auto on_unit = [&](const uint64_t* p) -> const uint64_t* { return ev + (size_t)(nat_of.at(p) - c0) * nb; };
-      for (u64 k = first_rebuilt; k < units_l; k++) {
-        BJ_TRY(lde_unit(ctx, mono, ev, log_n, log_l, cnt, k, 1));
-        for (const DeepGroup& g : deep_groups)
-          BJ_TRY(deep_range(g, [&](size_t i) { return in_chunk((*g.srcs)[i].c0); }, on_unit, k * nb, nb));
-      }
-      return BJ_OK;
-    }));
-  uint32_t new_pow = 0, num_queries = 0, sched[32], sched_len = 0, final_degree = 0;
-  BJ_TRY(bj_compute_fri_schedule(c.security_level, cap, c.pow_bits, log_l, log_n, &new_pow, &num_queries, sched, &sched_len, &final_degree));
-  bj_fri_oracles* fri = nullptr;
-  BJ_TRY(bj_do_fri_with_hasher(ctx, tr, (const uint64_t*)deep.p, (const uint64_t*)deep.p + nL, log_n + log_l, sched, sched_len, log_l, cap,
-                               c.tree_hasher, &fri));
-  struct FriGuard {
-    bj_fri_oracles* f;
-    ~FriGuard() { bj_fri_oracles_free(f); }
-  } frig{fri};
-  const uint32_t n_fri = bj_fri_oracles_num_oracles(fri);
-  pf->fri_caps.resize(n_fri);
-  for (uint32_t i = 0; i < n_fri; i++) {
-    pf->fri_caps[i].resize(4 * (size_t)cap);
-    BJ_TRY(bj_fri_oracles_get_cap(fri, i, (uint64_t*)pf->fri_caps[i].data()));
-  }
-  const uint32_t n_mono = bj_fri_oracles_num_monomials(fri);
-  pf->mono_c0.resize(n_mono);
-  pf->mono_c1.resize(n_mono);
-  BJ_TRY(bj_fri_oracles_get_monomials(fri, (uint64_t*)pf->mono_c0.data(), (uint64_t*)pf->mono_c1.data()));
-  if (new_pow) {  // prover.rs:2109-2132 with POW = Blake2s256: 5 challenges seed the search, the nonce re-enters the transcript
-    uint8_t seed[40];
-    for (int i = 0; i < 5; i++) {
-      const uint64_t e = bj_transcript_get_challenge(tr);
-      for (int k = 0; k < 8; k++) seed[8 * i + k] = (uint8_t)(e >> (8 * k));
-    }
-    uint64_t nonce = 0;
-    BJ_TRY(bj_pow_blake2s(ctx, seed, 40, new_pow, &nonce));
-    pf->pow_challenge = nonce;
-    const uint64_t lh[2] = {nonce & 0xffffffffull, nonce >> 32};
-    bj_transcript_witness_field_elements(tr, lh, 2);
-  }
+  BJ_TRY(p.deep_fri_pow());
   BJ_TRY(mark(4));
-
-  // ---- queries ----
-  const uint32_t max_bits = log_n + log_l;
-  std::vector<uint64_t> idxs(num_queries);
-  for (auto& i : idxs) i = bj_transcript_get_index_bits(tr, max_bits, max_bits);
-  pf->queries.assign(num_queries, {});
-  // a query is answered by the rank that owns the unit of its index (leaf t = coset * n + row lies in that rank's subtree);
-  // the other ranks look up a dummy leaf, the answers are exchanged and every rank keeps the owner's
-  std::vector<uint64_t> loc_idx(num_queries);
-  std::vector<uint32_t> owner(num_queries);
-  for (uint32_t q = 0; q < num_queries; q++) {
-    owner[q] = ctx->shard.owner(idxs[q], (int)log_n);
-    loc_idx[q] = owner[q] == rank ? ctx->shard.owner_index(idxs[q], (int)log_n) : 0;
-  }
-  // every answer part (leaf elements / path of one oracle) is gathered locally first; ONE exchange then carries all of them
-  struct Part {
-    std::vector<uint64_t> data;  // [num_queries][rec_len]
-    size_t rec_len;
-  };
-  std::vector<Part> parts;  // order: (rows, path) of the 4 base oracles, then (leaf elements, path) of every FRI level
-  const Oracle* base[4] = {&w_or, &s2_or, &qt_or, &setup->tree};
-  for (const Oracle* o : base) {
-    const size_t row_len = o->cols.size();
-    uint32_t depth = 0;
-    while ((o->n_leaves >> depth) > o->cap_size) depth++;
-    Part rows{std::vector<uint64_t>((size_t)num_queries * row_len), row_len};
-    Part path{std::vector<uint64_t>((size_t)num_queries * depth * 4), (size_t)depth * 4};
-    if (recompute && o != &qt_or) {
-      // no coset kept: every row is recomputed below
-    } else if (compact && o != &qt_or) {  // kept columns hold cosets [0, Q); the rows of the other cosets are recomputed below
-      std::vector<uint64_t> kept_idx(loc_idx);
-      for (auto& i : kept_idx)
-        if (i >= Qn) i = 0;
-      BJ_TRY(bj_query_leaf_elements(ctx, o->cols.data(), (uint32_t)row_len, 1, Qn, kept_idx.data(), num_queries, rows.data.data()));
-    } else {
-      BJ_TRY(bj_query_leaf_elements(ctx, o->cols.data(), (uint32_t)row_len, 1, o->n_leaves, loc_idx.data(), num_queries, rows.data.data()));
-    }
-    if (depth)
-      BJ_TRY(bj_merkle_paths(ctx, (const uint64_t*)o->leaf_hashes.p, (const uint64_t*)o->nodes.p, o->n_leaves, o->cap_size, loc_idx.data(),
-                             num_queries, path.data.data()));
-    parts.push_back(std::move(rows));
-    parts.push_back(std::move(path));
-  }
-  if (compact || recompute) {
-    // queries this context answers whose leaf lies in a local unit k >= first_rebuilt (a coset on one GPU): one recompute of
-    // each such unit per chunk, the queried rows gathered from it (the rows of every query, so that the gather buffer is the
-    // one the plan counts).  Natural column i belongs to the setup (rows in parts[6]), witness (parts[0]) or stage-2
-    // (parts[2]) oracle.  On a sharded context every rank runs the pass, also one that answers none of these queries: its
-    // peers are rebuilding meanwhile and the exchange waits for them, so it gathers from the chunk's monomials instead, and
-    // every rank's pool reaches the peak its plan counts.
-    const u32 log_nb = log_n - split;
-    std::vector<std::vector<uint32_t>> by_unit(units_l);
-    for (uint32_t q = 0; q < num_queries; q++)
-      if (owner[q] == rank && (loc_idx[q] >> log_nb) >= first_rebuilt) by_unit[loc_idx[q] >> log_nb].push_back(q);
-    bool any = false;
-    for (const auto& qs : by_unit) any = any || !qs.empty();
-    const uint32_t Wc = (uint32_t)w_or.cols.size();
-    if (any || world > 1)
-      BJ_TRY(for_chunks(0, (uint32_t)nat.size(), [&](uint32_t c0, uint32_t cnt, const uint64_t* mono, uint64_t* ev) -> int32_t {
-        std::vector<const uint64_t*> cols(cnt);
-        std::vector<uint64_t> rows_in(num_queries, 0), got((size_t)num_queries * cnt);
-        if (!any) {
-          for (uint32_t i = 0; i < cnt; i++) cols[i] = mono + (size_t)i * n;
-          return bj_query_leaf_elements(ctx, cols.data(), cnt, 1, n, rows_in.data(), num_queries, got.data());
-        }
-        for (uint32_t i = 0; i < cnt; i++) cols[i] = ev + (size_t)i * nb;
-        for (u64 k = first_rebuilt; k < units_l; k++) {
-          const auto& qs = by_unit[k];
-          if (qs.empty()) continue;
-          BJ_TRY(lde_unit(ctx, mono, ev, log_n, log_l, cnt, k, 1));
-          for (uint32_t q : qs) rows_in[q] = loc_idx[q] & (nb - 1);
-          BJ_TRY(bj_query_leaf_elements(ctx, cols.data(), cnt, 1, nb, rows_in.data(), num_queries, got.data()));
-          for (uint32_t i = 0; i < cnt; i++) {
-            const uint32_t col = c0 + i;
-            Part& pt = col < S ? parts[6] : col < S + Wc ? parts[0] : parts[2];
-            const uint32_t within = col < S ? col : col < S + Wc ? col - S : col - S - Wc;
-            for (uint32_t q : qs) pt.data[(size_t)q * pt.rec_len + within] = got[(size_t)q * cnt + i];
-          }
-        }
-        return BJ_OK;
-      }));
-  }
-  {
-    uint32_t log_len = log_n;  // coset length of the level's codeword
-    std::vector<uint64_t> sub(idxs);
-    for (uint32_t lvl = 0; lvl < sched_len; lvl++) {
-      const uint32_t k = sched[lvl];
-      const size_t le_len = (size_t)2 << k;
-      std::vector<uint64_t> locals(num_queries);
-      for (uint32_t q = 0; q < num_queries; q++) {
-        locals[q] = owner[q] == rank ? (ctx->shard.owner_index(sub[q], (int)log_len) >> k) : 0;
-        sub[q] >>= k;
-      }
-      uint32_t plen = 0;
-      Part les{std::vector<uint64_t>((size_t)num_queries * le_len, 0), le_len};
-      Part path{std::vector<uint64_t>((size_t)num_queries * 40 * 4, 0), 0};  // [num_queries][plen][4] after the call
-      BJ_TRY(bj_fri_oracles_query_batch(fri, lvl, locals.data(), num_queries, les.data.data(), path.data.data(), &plen));
-      path.rec_len = (size_t)plen * 4;
-      path.data.resize((size_t)num_queries * path.rec_len);
-      parts.push_back(std::move(les));
-      parts.push_back(std::move(path));
-      log_len -= k;
-    }
-  }
-  if (world > 1) {
-    size_t total = 0;
-    for (const auto& pt : parts) total += pt.data.size();
-    std::vector<uint64_t> mine(total), all((size_t)world * total);
-    size_t off = 0;
-    for (const auto& pt : parts) {
-      if (!pt.data.empty()) memcpy(mine.data() + off, pt.data.data(), sizeof(uint64_t) * pt.data.size());
-      off += pt.data.size();
-    }
-    BJ_TRY(comm_all_gather_host(ctx->comm, (const u64*)mine.data(), (u64*)all.data(), total));
-    off = 0;
-    for (auto& pt : parts) {
-      for (uint32_t q = 0; q < num_queries && pt.rec_len; q++)
-        memcpy(pt.data.data() + (size_t)q * pt.rec_len, all.data() + (size_t)owner[q] * total + off + (size_t)q * pt.rec_len,
-               sizeof(uint64_t) * pt.rec_len);
-      off += pt.data.size();
-    }
-  }
-  for (size_t o = 0; o + 1 < parts.size(); o += 2) {
-    const Part &le = parts[o], &pa = parts[o + 1];
-    for (uint32_t q = 0; q < num_queries; q++) {
-      QueryAnswer a;
-      a.leaf_elements.assign(le.data.begin() + (size_t)q * le.rec_len, le.data.begin() + (size_t)(q + 1) * le.rec_len);
-      a.path.assign(pa.data.begin() + (size_t)q * pa.rec_len, pa.data.begin() + (size_t)(q + 1) * pa.rec_len);
-      pf->queries[q].push_back(std::move(a));
-    }
-  }
+  BJ_TRY(p.queries());
   BJ_TRY(mark(5));
-
-  // ---- serde_json shape of Proof (proof.rs:57-143) ----
-  std::string& s = pf->json;
-  s.reserve(1 << 20);
-  const bool digest_bytes = c.tree_hasher != BJ_HASHER_POSEIDON2;
-  s += "{\"proof_config\":{\"fri_lde_factor\":" + std::to_string(L) + ",\"merkle_tree_cap_size\":" + std::to_string(cap) +
-       ",\"fri_folding_schedule\":null,\"security_level\":" + std::to_string(c.security_level) + ",\"pow_bits\":" + std::to_string(c.pow_bits) +
-       "},\"public_inputs\":";
-  json_u64_list(s, pf->public_inputs.data(), pf->public_inputs.size());
-  s += ",\"witness_oracle_cap\":";
-  json_digests(s, pf->witness_cap.data(), cap, digest_bytes);
-  s += ",\"stage_2_oracle_cap\":";
-  json_digests(s, pf->stage2_cap.data(), cap, digest_bytes);
-  s += ",\"quotient_oracle_cap\":";
-  json_digests(s, pf->quotient_cap.data(), cap, digest_bytes);
-  s += ",\"final_fri_monomials\":[";
-  json_u64_list(s, pf->mono_c0.data(), pf->mono_c0.size());
-  s += ',';
-  json_u64_list(s, pf->mono_c1.data(), pf->mono_c1.size());
-  s += "],\"values_at_z\":";
-  json_ext_list(s, pf->values_at_z);
-  s += ",\"values_at_z_omega\":";
-  json_ext_list(s, pf->values_at_z_omega);
-  s += ",\"values_at_0\":";
-  json_ext_list(s, pf->values_at_0);
-  s += ",\"fri_base_oracle_cap\":";
-  json_digests(s, pf->fri_caps[0].data(), cap, digest_bytes);
-  s += ",\"fri_intermediate_oracles_caps\":[";
-  for (uint32_t i = 1; i < n_fri; i++) {
-    if (i > 1) s += ',';
-    json_digests(s, pf->fri_caps[i].data(), cap, digest_bytes);
-  }
-  s += "],\"queries_per_fri_repetition\":[";
-  static const char* names[4] = {"witness_query", "stage_2_query", "quotient_query", "setup_query"};
-  auto json_answer = [&](const QueryAnswer& a) {
-    s += "{\"leaf_elements\":";
-    json_u64_list(s, a.leaf_elements.data(), a.leaf_elements.size());
-    s += ",\"proof\":";
-    json_digests(s, a.path.data(), a.path.size() / 4, digest_bytes);
-    s += '}';
-  };
-  for (uint32_t q = 0; q < num_queries; q++) {
-    if (q) s += ',';
-    s += '{';
-    for (int o = 0; o < 4; o++) {
-      s += std::string("\"") + names[o] + "\":";
-      json_answer(pf->queries[q][o]);
-      s += ',';
-    }
-    s += "\"fri_queries\":[";
-    for (uint32_t lvl = 0; lvl < sched_len; lvl++) {
-      if (lvl) s += ',';
-      json_answer(pf->queries[q][4 + lvl]);
-    }
-    s += "]}";
-  }
-  s += "],\"pow_challenge\":" + std::to_string(pf->pow_challenge) + ",\"_marker\":null}";
+  pf->json = proof_json(*pf, p.sched_len);
   *out = pf.release();
   return BJ_OK;
 }
@@ -1888,15 +1895,11 @@ static int32_t setup_shape(const bj_setup* s, ProofShape* sh) {
   return BJ_OK;
 }
 
-static MemoryPlan setup_plan_kind(const bj_setup* s) {
-  return s->compact ? PLAN_COMPACT : s->streamed ? PLAN_STREAMED : s->recompute ? PLAN_RECOMPUTE : PLAN_RESIDENT;
-}
-
 int32_t bj_proof_memory_plan_lanes(const bj_setup* setup, uint32_t n_lanes, uint64_t out[3]) {
   ProofShape sh;
   if (!setup || !out || n_lanes == 0 || comm_world(setup->ctx) != 1) return BJ_ERR_INVALID_ARG;
   BJ_TRY(setup_shape(setup, &sh));
-  lane_plan(sh, setup_plan_kind(setup), setup->chunk, n_lanes, out);
+  lane_plan(sh, setup->plan, setup->chunk, n_lanes, out);
   return BJ_OK;
 }
 
@@ -1905,7 +1908,7 @@ int32_t bj_proof_memory_plan_lane_pool(const bj_setup* setup, uint64_t* pool_byt
   if (!setup || !pool_bytes || comm_world(setup->ctx) != 1) return BJ_ERR_INVALID_ARG;
   BJ_TRY(setup_shape(setup, &sh));
   uint64_t out[3];
-  lane_plan(sh, setup_plan_kind(setup), setup->chunk, 1, out);
+  lane_plan(sh, setup->plan, setup->chunk, 1, out);
   *pool_bytes = out[1] - lane_reserve(sh);
   return BJ_OK;
 }
@@ -1929,7 +1932,7 @@ int32_t bj_ctx_create_lane(bj_ctx* parent, bj_ctx** out) {
       ProofShape sh;
       BJ_TRY(setup_shape(s, &sh));
       uint64_t p[3];
-      lane_plan(sh, setup_plan_kind(s), s->chunk, lanes_after + 1, p);
+      lane_plan(sh, s->plan, s->chunk, lanes_after + 1, p);
       const uint64_t limit = parent->memory_limit ? parent->memory_limit : s->limit;
       if (p[2] + lane_sets > limit)
         BJ_FAIL(parent, BJ_ERR_OOM, "bj_ctx_create_lane: the setup's plan needs " + std::to_string(s->chosen_bytes()) + " bytes and every lane " +
@@ -1942,11 +1945,11 @@ int32_t bj_ctx_create_lane(bj_ctx* parent, bj_ctx** out) {
   return ctx_new_lane(parent, out);
 }
 
-int32_t bj_setup_is_compact(const bj_setup* s) { return s ? (s->compact ? 1 : 0) : BJ_ERR_INVALID_ARG; }
+int32_t bj_setup_is_compact(const bj_setup* s) { return s ? (s->plan == PLAN_COMPACT ? 1 : 0) : BJ_ERR_INVALID_ARG; }
 
 int32_t bj_setup_plan(const bj_setup* s) {
   if (!s) return BJ_ERR_INVALID_ARG;
-  return s->compact ? BJ_PLAN_COMPACT : s->streamed ? BJ_PLAN_STREAMED : s->recompute ? BJ_PLAN_RECOMPUTE : BJ_PLAN_RESIDENT;
+  return s->plan;
 }
 
 int32_t bj_setup_row_blocks(const bj_setup* s) { return s ? (int32_t)(1u << s->log_blocks) : BJ_ERR_INVALID_ARG; }
@@ -1955,7 +1958,7 @@ int32_t bj_setup_memory_plan(const bj_setup* s, uint64_t out[3]) {
   if (!s || !out) return BJ_ERR_INVALID_ARG;
   out[0] = s->pool_bytes;
   out[1] = s->outside_pool_bytes;
-  out[2] = s->compact || s->recompute ? s->chunk : 0;
+  out[2] = s->plan == PLAN_COMPACT || s->plan == PLAN_RECOMPUTE ? s->chunk : 0;
   return BJ_OK;
 }
 

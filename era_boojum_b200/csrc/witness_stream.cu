@@ -215,7 +215,7 @@ static int32_t lane_witness_slots_reserve(bj_ctx* lane, const bj_setup* setup, u
   std::lock_guard<std::mutex> lock(parent->tables_mu);
   const uint32_t m = parent->lanes.load();
   uint64_t p[3];
-  lane_plan(sh, setup_plan_kind(setup), setup->chunk, m + 1, p);
+  lane_plan(sh, setup->plan, setup->chunk, m + 1, p);
   const uint64_t hint = max_values || setup->has_hint ? witness_hint_bytes(c) : 0;
   const uint64_t total = p[2] + hint + parent->witness_set_bytes + parent->lane_witness_set_bytes + own;
   const uint64_t limit = parent->memory_limit ? parent->memory_limit : setup->limit;
