@@ -845,3 +845,140 @@ API void orc_gates_check(const uint64_t *gates, size_t n_gates, const uint64_t *
   out[1] = failures ? first_key >> 32 : 0;
   out[2] = failures ? first_key & 0xffffffffu : 0;
 }
+
+/* ------------------------------------------------------------------------------------------------
+ * setup / witness materialisation (oracle/setup_oracle.py is the line-by-line Python restatement these are pinned to)
+ * ---------------------------------------------------------------------------------------------- */
+#define ORC_PLACEHOLDER_BIT (1ull << 63) /* Variable::placeholder       src/cs/mod.rs:44 */
+#define ORC_LOW_U48 ((1ull << 48) - 1)   /* LOW_U48_MASK                src/cs/mod.rs:47 */
+
+/* materialize_variables_polynomials_from_dense_hint        src/cs/implementations/witness.rs:325-385
+ * out [n_cols][2^log_n]: out[c][row] = all_values[hint[c][row]] mod p for row < hint_rows, 0 for placeholders and the rows
+ * past the hint.  The index is the Variable's low 48 bits (the reference indexes with the whole word, which is the same for
+ * every Variable it creates).  Returns the number of non-placeholder cells whose index is >= n_values (those stay 0). */
+API uint64_t orc_materialize_columns(const uint64_t *values, size_t n_values, const uint64_t *hint, size_t n_cols, size_t hint_rows,
+                                     unsigned log_n, uint64_t *out) {
+  const size_t n = (size_t)1 << log_n;
+  uint64_t bad = 0;
+#pragma omp parallel for schedule(static) reduction(+ : bad)
+  for (long cl = 0; cl < (long)n_cols; cl++) {
+    const size_t c = (size_t)cl;
+    for (size_t row = 0; row < n; row++) {
+      uint64_t v = 0;
+      if (row < hint_rows) {
+        const uint64_t h = hint[c * hint_rows + row];
+        if (!(h & ORC_PLACEHOLDER_BIT)) {
+          if ((h & ORC_LOW_U48) < n_values) v = gl_canon(values[h & ORC_LOW_U48]);
+          else bad++;
+        }
+      }
+      out[c * n + row] = v;
+    }
+  }
+  return bad;
+}
+
+/* the per-variable scratch of create_permutation_polys, a HashMap<Variable, (F, (usize, usize))> in the reference: open
+ * addressing with linear probing, keyed by the variable index (an empty slot holds ~0, which no 48-bit index equals).  One
+ * entry holds all a visit touches, so a visit costs one cache miss, and the walk prefetches the entries of the cells ahead. */
+typedef struct {
+  uint64_t key, value, first; /* variable index, the value it carries, the flat cell of its first occurrence */
+} orc_scratch_entry;
+
+typedef struct {
+  orc_scratch_entry *e;
+  size_t cap, count;
+} orc_scratch;
+
+static inline size_t scratch_home(const orc_scratch *s, uint64_t key) {
+  return (size_t)((key * 0x9E3779B97F4A7C15ull) >> 20) & (s->cap - 1);
+}
+
+static size_t scratch_slot(const orc_scratch *s, uint64_t key) {
+  size_t i = scratch_home(s, key);
+  while (s->e[i].key != ~0ull && s->e[i].key != key) i = (i + 1) & (s->cap - 1);
+  return i;
+}
+
+static int scratch_alloc(orc_scratch *s, size_t cap) {
+  s->cap = cap;
+  s->count = 0;
+  s->e = malloc(sizeof(orc_scratch_entry) * cap);
+  if (!s->e) return -1;
+#pragma omp parallel for schedule(static)
+  for (long i = 0; i < (long)cap; i++) s->e[i].key = ~0ull;
+  return 0;
+}
+
+/* doubles the table once it is three quarters full */
+static int scratch_grow(orc_scratch *s) {
+  orc_scratch t;
+  if (scratch_alloc(&t, s->cap * 2)) return -1;
+  for (size_t i = 0; i < s->cap; i++)
+    if (s->e[i].key != ~0ull) t.e[scratch_slot(&t, s->e[i].key)] = s->e[i];
+  t.count = s->count;
+  free(s->e);
+  *s = t;
+  return 0;
+}
+
+/* create_permutation_polys                                 src/cs/implementations/setup.rs:419-502
+ * placement [n_cols][2^log_n] Variables (copy_permutation_data), non_residues [n_cols] (non_residues_for_copy_permutation),
+ * out [n_cols][2^log_n] the sigma columns.  out starts as the identity k_c * w^row (materialize_x_by_non_residue_polys);
+ * the cells are visited column by column, row by row, and each occurrence of a variable swaps its value with the variable's
+ * scratch value (:446-473); at the end every variable's scratch value goes to its first occurrence (:476-489).  Returns 0,
+ * or -1 when the scratch table cannot be allocated. */
+API int orc_create_permutation_polys(const uint64_t *placement, size_t n_cols, unsigned log_n, const uint64_t *non_residues,
+                                     uint64_t *out) {
+  const size_t n = (size_t)1 << log_n, cells = n * n_cols;
+  const uint64_t w = gl_omega(log_n);
+  uint64_t *pows = malloc(sizeof(uint64_t) * n);
+  if (!pows) return -1;
+#pragma omp parallel for schedule(static)
+  for (long rl = 0; rl < (long)n; rl += 4096) {
+    uint64_t x = gl_pow(w, (uint64_t)rl);
+    for (size_t row = (size_t)rl; row < (size_t)rl + 4096 && row < n; row++) {
+      pows[row] = x;
+      x = gl_mul(x, w);
+    }
+  }
+#pragma omp parallel for schedule(static)
+  for (long cl = 0; cl < (long)n_cols; cl++) {
+    const size_t c = (size_t)cl;
+    const uint64_t k = gl_canon(non_residues[c]);
+    for (size_t row = 0; row < n; row++) out[c * n + row] = gl_mul(k, pows[row]);
+  }
+  free(pows);
+  /* sized for a variable per two cells, about what a circuit has; the table grows past that */
+  size_t cap = 1 << 16;
+  while (cap < cells / 2) cap *= 2;
+  orc_scratch s;
+  if (scratch_alloc(&s, cap)) return -1;
+  enum { AHEAD = 16 };
+  for (size_t cell = 0; cell < cells; cell++) {
+    if (cell + AHEAD < cells) __builtin_prefetch(&s.e[scratch_home(&s, placement[cell + AHEAD] & ORC_LOW_U48)], 1);
+    const uint64_t var = placement[cell];
+    if (var & ORC_PLACEHOLDER_BIT) continue;
+    const uint64_t idx = var & ORC_LOW_U48;
+    size_t i = scratch_slot(&s, idx);
+    if (s.e[i].key == idx) {
+      const uint64_t t = s.e[i].value;
+      s.e[i].value = out[cell];
+      out[cell] = t;
+      continue;
+    }
+    if (4 * (s.count + 1) > 3 * s.cap) {
+      if (scratch_grow(&s)) {
+        free(s.e);
+        return -1;
+      }
+      i = scratch_slot(&s, idx);
+    }
+    s.e[i] = (orc_scratch_entry){idx, out[cell], cell};
+    s.count++;
+  }
+  for (size_t i = 0; i < s.cap; i++)
+    if (s.e[i].key != ~0ull) out[s.e[i].first] = s.e[i].value;
+  free(s.e);
+  return 0;
+}

@@ -65,6 +65,8 @@ def lib():
             "orc_horner_ext": (None, [vp, sz, sz, vp, vp]),
             "orc_gates_quotient": (None, [vp, sz, vp, vp, vp, ctypes.c_uint32, ctypes.c_uint32, vp, sz, vp, vp]),
             "orc_gates_check": (None, [vp, sz, vp, vp, vp, ctypes.c_uint32, sz, vp, vp, vp]),
+            "orc_materialize_columns": (u64, [vp, sz, vp, sz, sz, ctypes.c_uint, vp]),
+            "orc_create_permutation_polys": (ctypes.c_int, [vp, sz, ctypes.c_uint, vp, vp]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)
@@ -464,3 +466,27 @@ def gates_report(gates, variables, constants):
         rep.update(gate_row=row, gate_index=gi, gate_repetition=(t - base) // len(g["writes"]), gate_term=(t - base) % len(g["writes"]),
                    gate_value=int(c["first_value"][row]), gate_selector=int(c["first_selector"][row]))
     return rep
+
+
+# ------------------------------------------------------------- setup / witness columns -----
+def materialize_columns(all_values, hint, log_n):
+    """materialize_variables_polynomials_from_dense_hint (cs/implementations/witness.rs:325-385).  all_values [n_values],
+    hint [n_cols, hint_rows] of `Variable`s (bit 63 = placeholder) -> (columns [n_cols, 2^log_n], number of non-placeholder
+    cells whose index is past all_values; those cells stay 0)."""
+    v, h = _u64(all_values), _u64(hint)
+    out = np.empty((h.shape[0], 1 << log_n), np.uint64)
+    bad = lib().orc_materialize_columns(_p(v), v.size, _p(h), h.shape[0], h.shape[1], log_n, _p(out))
+    return out, int(bad)
+
+
+def create_permutation_polys(placement):
+    """create_permutation_polys (cs/implementations/setup.rs:419-502).  placement [n_cols, n] of `Variable`s
+    (copy_permutation_data) -> the sigma columns [n_cols, n]."""
+    from .stage2 import non_residues_for_copy_permutation
+    pl = _u64(placement)
+    n_cols, n = pl.shape
+    nr = _u64(non_residues_for_copy_permutation(n, n_cols))
+    out = np.empty((n_cols, n), np.uint64)
+    if lib().orc_create_permutation_polys(_p(pl), n_cols, n.bit_length() - 1, _p(nr), _p(out)):
+        raise MemoryError("orc_create_permutation_polys: the scratch table does not fit in host memory")
+    return out

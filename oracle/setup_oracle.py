@@ -1,5 +1,7 @@
 """TEST ORACLE (never imported by the product): Python restatement of the reference's host loops that build the witness
-columns and the sigma columns.  Follows the reference line by line; small sizes only.
+columns and the sigma columns.  Follows the reference line by line; small sizes only (oracle.c's orc_materialize_columns and
+orc_create_permutation_polys restate the same loops for production sizes and are pinned to these by
+tests/test_setup_oracle_cpu.py).
 
   materialize_variables_polynomials_from_dense_hint   src/cs/implementations/witness.rs:325-385
   create_permutation_polys                            src/cs/implementations/setup.rs:419-502

@@ -214,7 +214,9 @@ def test_lde_prover_shape_2pow22_factor8_vs_oracle(bj, ctx):
 
 # ------------------------------------------------------------------------------------ Poseidon2 / Merkle -----
 def test_poseidon2_permutation_matches_oracle(bj, ctx):
-    st = rng(8).integers(0, 2**64, size=(300, 12), dtype=np.uint64)  # includes non-canonical values
+    r = rng(8)
+    st = r.integers(0, 2**64, size=(300, 12), dtype=np.uint64)
+    st[::7, ::3] = r.integers(P, 2**64, size=st[::7, ::3].shape, dtype=np.uint64)  # non-canonical words in the checked rows
     d = bj.to_device(st)
     ctx.poseidon2_permute(d)
     got = bj.to_numpy(d)
@@ -972,7 +974,8 @@ def test_materialize_columns_and_permutation_polys_match_reference_loops(bj, ctx
     hint_rows = n - 3
     place = rng.integers(0, n_vars, size=(n_cols, n), dtype=np.uint64)
     place[rng.random((n_cols, n)) < 0.2] = SO.PLACEHOLDER_BIT          # unassigned cells
-    values = rng.integers(0, 2**64 - 1, size=n_vars, dtype=np.uint64)  # incl. non-canonical values
+    values = rng.integers(0, 2**64 - 1, size=n_vars, dtype=np.uint64)
+    values[::3] = rng.integers(P, 2**64, size=values[::3].shape, dtype=np.uint64)  # non-canonical words
     hint = np.ascontiguousarray(place[:, :hint_rows])
     got = bj.to_numpy(c.materialize_variables_polynomials_from_dense_hint(bj.to_device(values), bj.to_device(hint), log_n))
     want = SO.materialize_columns([int(v) for v in values], [[int(v) for v in col] for col in hint], n)
