@@ -90,6 +90,7 @@ int32_t ctx_new_lane(bj_ctx* parent, bj_ctx** out) {
   lane->ntt_pass1_w = parent->ntt_pass1_w;
   lane->ntt_chunk_mb = parent->ntt_chunk_mb;
   lane->ntt_full_pow = parent->ntt_full_pow;
+  lane->ntt_twist = parent->ntt_twist;
   lane->gate_peephole = parent->gate_peephole;
   lane->gate_points_per_thread = parent->gate_points_per_thread;
   lane->ntt_l2_persist = 0;  // the carve-out is sized for one stream's table (ctx.hpp)
@@ -198,6 +199,7 @@ int32_t bj_ctx_create(int32_t device, void* stream, bj_ctx** out_ctx) {
   ctx->ntt_use_v2 = env_int("BJ_NTT_V2", 1);
   ctx->ntt_col_fastest = env_int("BJ_NTT_COL_FASTEST", -1);
   ctx->ntt_full_pow = env_int("BJ_NTT_FULL_POW", 1);
+  ctx->ntt_twist = env_int("BJ_NTT_TWIST", 1);
   ctx->ntt_bulk = env_int("BJ_NTT_BULK", 0);
   ctx->ntt_l2_persist = env_int("BJ_NTT_L2_PERSIST", 1);
   ctx->ntt_chunk_mb = env_int("BJ_NTT_CHUNK_MB", 0);
@@ -236,6 +238,7 @@ int32_t bj_ctx_destroy(bj_ctx* ctx) {
     cudaFree(e.hi);
     if (e.full) cudaFree(e.full);
   }
+  for (auto& e : ctx->twist_cache) cudaFree(e.tab);
   for (void* p : ctx->tables_retired) cudaFree(p);
   if (ctx->pow_best) cudaFree(ctx->pow_best);
   if (ctx->gate_program) cudaFree(ctx->gate_program);

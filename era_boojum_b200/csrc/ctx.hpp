@@ -26,6 +26,13 @@ struct PowTab {
   u64* full;  // s * c^i for all i < 2^log_n, or nullptr (built while the per-context budget lasts)
 };
 
+// a forward coset transform's twiddles with the coset folded in (ntt.cu get_twist_table): tab[2^r + G], 2^log_n entries
+struct TwistTab {
+  u64 coset;
+  int log_n;
+  u64* tab;
+};
+
 // Domain shard of a multi-GPU prover, the one owner of the layout rule.  The LDE domain is cut into UNITS u = j * B + p,
 // B = 2^log_split: row block p (rows [p n / B, (p + 1) n / B) of the coset's bit-reversed row order) of coset j, so the flat
 // index of a domain point is t = u * (n / B) + i'.  LDE-domain buffers of this context hold only the units
@@ -104,7 +111,8 @@ struct bj_ctx {
   bj::u64* tw_inv = nullptr;
   int tw_log = 0;  // tables hold 2^(tw_log-1) entries
   std::vector<bj::PowTab> pow_cache;
-  size_t pow_full_bytes = 0;  // bytes held by the full power tables of pow_cache
+  std::vector<bj::TwistTab> twist_cache;
+  size_t pow_full_bytes = 0;  // bytes held by the full power tables of pow_cache and the tables of twist_cache
   void* scratch = nullptr;
   size_t scratch_bytes = 0;
   void* ptr_table = nullptr;  // device copy of host pointer arrays (Merkle sources)
@@ -136,7 +144,8 @@ struct bj_ctx {
   int ntt_max_tile_log = 13;  // tunables (env BJ_NTT_*)
   int ntt_pass1_w = -1;
   int ntt_chunk_mb = 0;
-  int ntt_full_pow = 1;          // BJ_NTT_FULL_POW=0 keeps the two-level coset power tables only
+  int ntt_full_pow = 1;          // BJ_NTT_FULL_POW=0 keeps the two-level coset power tables only (no expanded, no twisted table)
+  int ntt_twist = 1;             // BJ_NTT_TWIST=0: forward coset transforms scale on load instead of using twisted twiddles
   uint32_t one = 1;              // a 1 the compiler cannot see (passed as a kernel parameter): additions written as multiply-adds by it issue on the FMA pipe (blake2s.cu)
   int gate_peephole = 15;          // BJ_GATE_PEEPHOLE: bit 0 = alias x*1 / x+0 / x*0, 1 = multiply-add fusion, 2 = linear combinations, 3 = pushing steps (gates.cu)
   int gate_points_per_thread = 0;  // BJ_GATE_POINTS_PER_THREAD=1|2|4: force the gate interpreter's points per thread (0: by size)
@@ -161,7 +170,7 @@ struct bj_ctx {
   //    than that pair makes the lane build a private pair (own_twiddles, freed with the lane).  A lane never grows the
   //    parent's pair.  The parent grows its own pair under tables_mu and, while it has lanes, retires the replaced pair
   //    (tables_retired, freed with the parent) instead of freeing it, so a lane's view stays valid.
-  //  - coset-power tables: the parent's pow_cache, shared.  Every lookup and insert, the parent's too, holds the parent's
+  //  - coset-power and twisted twiddle tables: the parent's pow_cache and twist_cache, shared.  Every lookup and insert, the parent's too, holds the parent's
   //    tables_mu.  A missing table is built on the caller's stream and, when a lane could read it, that stream is
   //    synchronised before the table is published, so a published table is complete.  While the parent has lanes its cache
   //    is never flushed: the 64-entry flush retires the tables instead.  The 3 GiB budget of full tables is the parent's.
@@ -180,7 +189,7 @@ struct bj_ctx {
   // Teardown: bj_ctx_destroy refuses a context with lanes alive, and a lane with slot sets alive; sets go first, then lanes.
   bj_ctx* parent = nullptr;       // a lane's parent (nullptr: a context of bj_ctx_create)
   std::atomic<uint32_t> lanes{0};  // lanes of this context alive
-  std::mutex tables_mu;            // guards tw_*, pow_cache, pow_full_bytes, tables_retired, setups and the set counts (see above)
+  std::mutex tables_mu;            // guards tw_*, pow_cache, twist_cache, pow_full_bytes, tables_retired, setups and the set counts (see above)
   std::vector<void*> tables_retired;
   bool own_twiddles = true;        // false while a lane's tw_* view the parent's pair
   std::vector<const bj_setup*> setups;  // setups alive on this context: bj_ctx_create_lane plans against them

@@ -101,7 +101,7 @@ __global__ void __launch_bounds__(512) ntt_pass_kernel(const NttPass p) {
     const int pp = b_lo + w - (4 - rs);  // position of the 4 thread-local index bits
     for (int q = tid; q < nvt; q += nthr) {
       const int e0 = ((q >> pp) << (pp + 4)) | (q & ((1 << pp) - 1));
-      u32 hq = hi;
+      u32 hq = hi | p.tw_prefix;  // twisted table: round rho's twiddles start at tab + 2^rho (ntt.cuh)
       if (p.kind != PASS_TILE) {
         const u32 k1 = (u32)(tile << w) + (e0 & (W - 1));
         hq = r0 ? (__brev(k1) >> (32 - r0)) : 0u;
@@ -215,6 +215,18 @@ __global__ void pow_table_kernel(u64* out, u32 count, int bits, PowSquares ps, u
   out[i] = gl::canon(r);
 }
 
+// tw[2^r + G] = tab[G] * c^(2^(log_n - r - 1)) for r < log_n, G < 2^r (tw[0] is not read); ps.sq[b] = c^(2^b)
+__global__ void twist_table_kernel(u64* tw, u32 count, int log_n, const u64* __restrict__ tab, PowSquares ps) {
+  const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  if (i == 0) {
+    tw[0] = 0;
+    return;
+  }
+  const int r = 31 - __clz(i);
+  tw[i] = gl::canon(gl::mul(__ldg(tab + (i - (1u << r))), ps.sq[log_n - r - 1]));
+}
+
 __global__ void bitreverse_kernel(u64* data, u64 col_stride, int log_n) {
   const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (1ull << log_n)) return;
@@ -255,17 +267,24 @@ static PowSquares make_squares(u64 w) {
   return ps;
 }
 
+// bytes of the n-entry tables the owner's caches hold: the expanded coset powers of pow_cache and the twisted tables
+static size_t cached_full_bytes(const bj_ctx* owner) {
+  size_t b = 0;
+  for (const auto& e : owner->pow_cache)
+    if (e.full) b += sizeof(u64) << e.log_n;
+  for (const auto& e : owner->twist_cache) b += sizeof(u64) << e.log_n;
+  return b;
+}
+
 // a parent whose lanes are all gone frees the tables it retired while they lived.  Called on the parent's own thread under its
 // tables_mu, after its stream has drained: no lane is left to read them (bj_ctx_destroy synchronised each lane's stream) and
-// the parent's earlier kernels are done.  The full-table budget is then recounted from the cache.
+// the parent's earlier kernels are done.  The full-table budget is then recounted from the caches.
 static int32_t release_retired(bj_ctx* owner) {
   if (owner->tables_retired.empty() || owner->lanes.load() > 0) return BJ_OK;
   BJ_CUDA(owner, cudaStreamSynchronize(owner->stream));
   for (void* p : owner->tables_retired) cudaFree(p);
   owner->tables_retired.clear();
-  owner->pow_full_bytes = 0;
-  for (const auto& e : owner->pow_cache)
-    if (e.full) owner->pow_full_bytes += sizeof(u64) << e.log_n;
+  owner->pow_full_bytes = cached_full_bytes(owner);
   return BJ_OK;
 }
 
@@ -358,7 +377,7 @@ static int32_t get_pow_tables(bj_ctx* ctx, u64 c, int log_n, u64 scale, PowTab* 
       if (e.full) cudaFree(e.full);
     }
     owner->pow_cache.clear();
-    if (!shared) owner->pow_full_bytes = 0;  // retired full tables count against the budget until release_retired
+    if (!shared) owner->pow_full_bytes = cached_full_bytes(owner);  // retired full tables count against the budget until release_retired
   }
   PowTab pt;
   pt.coset = c;
@@ -393,6 +412,52 @@ static int32_t get_pow_tables(bj_ctx* ctx, u64 c, int log_n, u64 scale, PowTab* 
 }
 
 int32_t get_pow_tables_public(bj_ctx* ctx, u64 c, int log_n, u64 scale, PowTab* out) { return get_pow_tables(ctx, c, log_n, scale, out); }
+
+// The forward transform on the coset c w^k evaluates a mod (X^n - c^n): round r splits X^(n/2^r) - c^(n/2^r) w_G into
+// X^(n/2^(r+1)) -+ c^(n/2^(r+1)) tab[G], so the coset folds into the twiddles, tab_c[2^r + G] = tab[G] c^(2^(log_n - r - 1)),
+// and the outputs are the same points in the same bit-reversed order with no per-element scaling.  One table of 2^log_n
+// entries per (c, log_n), cached on the owner context with the rules of the coset-power tables (ctx.hpp) and counted against
+// their budget; *out = nullptr when the budget is spent, and the caller scales on load instead.  ctx's twiddles must cover
+// log_n (ensure_twiddles).
+// The price is the front pass's FIRST stage (group 0's twiddle is no longer 1): 0.5-0.94 multiplications per element against
+// the 1 multiplication and 8-byte table read of the scale.  From 2^13 on (multi-pass plans) that pays; a one-pass transform
+// up to 2^12 keeps scaling on load, where the two are about even and a table per (coset, size) would only fill the cache.
+static constexpr int TWIST_MIN_LOG = 13;
+static int32_t get_twist_table(bj_ctx* ctx, u64 c, int log_n, const u64** out) {
+  *out = nullptr;
+  bj_ctx* owner = ctx->parent ? ctx->parent : ctx;
+  std::lock_guard<std::mutex> lock(owner->tables_mu);
+  if (owner == ctx) BJ_TRY(release_retired(ctx));
+  for (const auto& e : owner->twist_cache)
+    if (e.coset == c && e.log_n == log_n) {
+      *out = e.tab;
+      return BJ_OK;
+    }
+  const bool shared = owner->lanes.load() > 0;
+  if (owner->twist_cache.size() >= 64) {  // bounded cache, as get_pow_tables
+    BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    for (auto& e : owner->twist_cache) {
+      if (shared) owner->tables_retired.push_back(e.tab);
+      else cudaFree(e.tab);
+    }
+    owner->twist_cache.clear();
+    if (!shared) owner->pow_full_bytes = cached_full_bytes(owner);
+  }
+  const size_t bytes = sizeof(u64) << log_n;
+  TwistTab tt{c, log_n, nullptr};
+  if (owner->pow_full_bytes + bytes > POW_FULL_BUDGET || cudaMalloc(&tt.tab, bytes) != cudaSuccess) {
+    cudaGetLastError();
+    return BJ_OK;
+  }
+  const u32 count = 1u << log_n;
+  twist_table_kernel<<<(count + 255) / 256, 256, 0, ctx->stream>>>(tt.tab, count, log_n, ctx->tw_fwd, make_squares(c));
+  BJ_LAUNCH_CHECK(ctx);
+  owner->pow_full_bytes += bytes;
+  if (shared) BJ_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // complete before another stream can read it
+  owner->twist_cache.push_back(tt);
+  *out = tt.tab;
+  return BJ_OK;
+}
 
 // The largest plan of any allowed tile setting (BJ_NTT_MAX_TILE_LOG 8..14) up to log_n = 32: an inverse of 2^31 or 2^32
 // with 2^8-value tiles takes 6 passes (tools/ntt_model.py enumerates them).
@@ -521,7 +586,8 @@ static int32_t launch_pass(bj_ctx* ctx, const NttPass& p, u32 n_cols) {
 
 // One batched transform.  src may equal dst for forward; the natural->natural inverse with more than one
 // pass needs `scratch` (n_cols * n elements) because its last pass cannot run in place.
-//   forward: coset scaling on load of the first pass; inverse: n^-1 coset^-i on the store of the last pass.
+//   forward: the coset's twisted twiddles (get_twist_table), or where there are none coset scaling on load of the first
+//   pass; inverse: n^-1 coset^-i on the store of the last pass.
 static int32_t run_transform(bj_ctx* ctx, const u64* src, u64 src_stride, u64* dst, u64 dst_stride, int m,
                              u32 n_cols, u64 coset, bool inverse, u64* scratch, u64 scratch_stride) {
   BJ_TRY(ensure_twiddles(ctx, m));
@@ -544,8 +610,11 @@ static int32_t run_transform(bj_ctx* ctx, const u64* src, u64 src_stride, u64* d
   PowTab pt{};
   int scale_mode = SCALE_NONE;
   u64 scale_const = 1;
+  const u64* twist = nullptr;
   if (!inverse) {
-    if (coset != 1) {
+    // a coset from 2^TWIST_MIN_LOG on: the coset's twisted twiddles (get_twist_table), no scaling; while their budget lasts
+    if (coset != 1 && ctx->ntt_twist && ctx->ntt_full_pow && m >= TWIST_MIN_LOG) BJ_TRY(get_twist_table(ctx, coset, m, &twist));
+    if (coset != 1 && !twist) {
       BJ_TRY(get_pow_tables(ctx, coset, m, 1, &pt));
       scale_mode = SCALE_POW;
     }
@@ -565,7 +634,8 @@ static int32_t run_transform(bj_ctx* ctx, const u64* src, u64 src_stride, u64* d
   for (int i = 0; i < pl.n_pass; i++) {
     const bool first = i == 0, last = i == pl.n_pass - 1;
     NttPass p{};
-    p.tab = tab;
+    p.tab = twist ? twist : tab;
+    p.tw_prefix = twist ? 1u << r0 : 0u;
     p.log_n = m;
     p.r0 = r0;
     p.t = pl.t[i];

@@ -37,6 +37,9 @@ struct NttPass {
   int pw_split;
   const u64* pw_full;  // SCALE_FULL: s * c^i for every i < 2^log_n (one load, one multiplication per element)
   int canon_out;       // canonicalise values at the store (last pass)
+  // PASS_TILE with a coset's twisted table as tab (forward coset transform, run_transform): 2^r0, else 0.  The twiddles of
+  // round rho start at tab + 2^rho, so the kernels put this 1 above the r0 prefix bits of the tile's twiddle index
+  unsigned tw_prefix;
   // specialised PASS_TILE kernels on a one-dimensional grid (n_cols > 0): block w is the tile w / n_cols of column
   // w % n_cols (column-fastest: the same tile of every column back to back); n_cols == 0: grid (tile, column)
   unsigned n_cols;

@@ -202,8 +202,12 @@ __device__ __forceinline__ void ntt_pass_v2_body(const NttPass& p) {
   }
   __syncthreads();
 
-  if (r0 == 0) v2_stage<T, W, KIND, 0, true>(sm, p.tab, tid, hi, tile, r0);
-  else v2_stage<T, W, KIND, 0, false>(sm, p.tab, tid, hi, tile, r0);
+  // a twisted table (PASS_TILE): the tile's twiddle prefix gets the leading 1 that selects round rho's slice tab + 2^rho, and
+  // group 0's twiddle is a coset power, not 1, so the FIRST stage does not apply
+  const u32 tw_prefix = KIND == PASS_TILE ? p.tw_prefix : 0u;
+  const u32 hs = hi | tw_prefix;
+  if ((r0 | tw_prefix) == 0) v2_stage<T, W, KIND, 0, true>(sm, p.tab, tid, hs, tile, r0);
+  else v2_stage<T, W, KIND, 0, false>(sm, p.tab, tid, hs, tile, r0);
 
   if constexpr (KIND == PASS_TILE) {
 #pragma unroll 4
@@ -323,8 +327,8 @@ __global__ void __launch_bounds__(V2Cfg<T, 0>::THREADS) ntt_pass_bulk_kernel(con
     sm[pe + 1] = v.y;
   }
   __syncthreads();
-  if (p.r0 == 0) v2_stage<T, 0, PASS_TILE, 0, true>(sm, p.tab, tid, tile, tile, p.r0);
-  else v2_stage<T, 0, PASS_TILE, 0, false>(sm, p.tab, tid, tile, tile, p.r0);
+  if ((p.r0 | p.tw_prefix) == 0) v2_stage<T, 0, PASS_TILE, 0, true>(sm, p.tab, tid, tile, tile, p.r0);
+  else v2_stage<T, 0, PASS_TILE, 0, false>(sm, p.tab, tid, tile | p.tw_prefix, tile, p.r0);
 #pragma unroll 4
   for (int pi = tid; pi < C::E / 2; pi += C::THREADS) {
     const int pe = v2_phys(2 * pi);

@@ -30,6 +30,17 @@ def twiddle_table(log_n, inverse):
     return [pow(w, brev(k, bits), P) for k in range(1 << bits)] if log_n >= 1 else [1]
 
 
+def twist_table(log_n, coset):
+    """ntt.cu get_twist_table: tw[2^r + G] = tab[G] * coset^(2^(log_n - r - 1)), r < log_n, G < 2^r (tw[0] unused)."""
+    tab = twiddle_table(log_n, False)
+    tw = [0] * (1 << log_n)
+    for r in range(log_n):
+        c = pow(coset, 1 << (log_n - r - 1), P)
+        for g in range(1 << r):
+            tw[(1 << r) + g] = tab[g] * c % P
+    return tw
+
+
 NTT_MAX_PASSES = 6  # capacity of ntt.cu's Plan
 
 
@@ -58,8 +69,9 @@ def make_plan(m, transpose_last, MAXE=13, pass1_w=-1):
     return plan
 
 
-def run_pass(src, m, r0, t, w, kind, tab, scale=None, scale_on_load=True):
-    """kind 0 = PASS_TILE, 1 = PASS_TRANSPOSE_LAST.  scale: function(index) -> factor or None."""
+def run_pass(src, m, r0, t, w, kind, tab, scale=None, scale_on_load=True, twisted=False):
+    """kind 0 = PASS_TILE, 1 = PASS_TRANSPOSE_LAST.  scale: function(index) -> factor or None.  twisted (PASS_TILE): tab
+    is a twist_table, round rho's twiddles start at tab[2^rho]."""
     LOG_E = t + w
     E, W = 1 << LOG_E, 1 << w
     dst = [None] * (1 << m)
@@ -102,7 +114,7 @@ def run_pass(src, m, r0, t, w, kind, tab, scale=None, scale_on_load=True):
             assert pp >= 0
             for q in range(nvt):
                 e0 = ((q >> pp) << (pp + 4)) | (q & ((1 << pp) - 1))
-                hq = hi
+                hq = (hi | (1 << r0)) if twisted else hi
                 if kind != 0:
                     k1 = (tile << w) + (e0 & (W - 1))
                     hq = brev(k1, r0) if r0 else 0
@@ -146,14 +158,16 @@ def run_pass(src, m, r0, t, w, kind, tab, scale=None, scale_on_load=True):
     return dst
 
 
-def transform(a, coset=1, inverse=False, MAXE=13, pass1_w=-1):
+def transform(a, coset=1, inverse=False, MAXE=13, pass1_w=-1, twist=False):
+    """twist (forward, coset != 1): the coset folded into the twiddles (twist_table), no scaling."""
     a = [int(x) % P for x in a]
     m = len(a).bit_length() - 1
     assert m >= 4
-    tab = twiddle_table(m, inverse)
+    twisted = twist and not inverse and coset != 1
+    tab = twist_table(m, coset) if twisted else twiddle_table(m, inverse)
     plan = make_plan(m, inverse, MAXE, pass1_w)
     if not inverse:
-        scale = (lambda i: pow(coset, i, P)) if coset != 1 else None
+        scale = (lambda i: pow(coset, i, P)) if coset != 1 and not twisted else None
     else:
         n_inv = pow(1 << m, P - 2, P)
         cinv = pow(coset, P - 2, P)
@@ -167,6 +181,6 @@ def transform(a, coset=1, inverse=False, MAXE=13, pass1_w=-1):
             sc, on_load = scale, True
         if inverse and last:
             sc, on_load = scale, False
-        cur = run_pass(cur, m, r0, t, w, kind, tab, sc, on_load)
+        cur = run_pass(cur, m, r0, t, w, kind, tab, sc, on_load, twisted)
         r0 += t
     return np.array(cur, dtype=np.uint64), plan
